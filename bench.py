@@ -25,16 +25,6 @@ METRIC = "audio-seconds/sec at preset='standard'"
 UNIT = "audio-s/s"
 
 
-def ncu_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the probed kernels, parsed from the committed ncu
-    --set full captures by tools/ncu_traffic.py into profiles/ncu_traffic.json ({probe-name prefix: {bytes, source}})."""
-    p = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if not os.path.exists(p):
-        return {}
-    with open(p) as f:
-        return json.load(f)
-
-
 def load_tokens(name="para53"):
     with open(os.path.join(ROOT, "tests", "golden", "bench_text_tokens.json")) as f:
         return json.load(f)[name]["tokens"]
@@ -80,11 +70,9 @@ def progress(msg):
 
 
 def peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return d["hbm_gbs"], d.get("bf16_tflops_sustained", d["bf16_tflops"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, 1400.0, "fallback (B200_PROFILING.md)"
+    """HBM GB/s and dense bf16 TFLOP/s the kernel probes are rated against: NVIDIA's data sheet for the H100 SXM at its
+    700 W limit (a card set to a lower power limit sustains less; the run's clocks are in the "clocks" field)."""
+    return 3350.0, 989.0, "H100 SXM data sheet"
 
 
 def kernel_probes(tts, cfg, n_mel, B, P, iters=200):
@@ -103,7 +91,7 @@ def kernel_probes(tts, cfg, n_mel, B, P, iters=200):
         ts = []
         for _ in range(reps):
             if flush is not None:
-                flush.zero_()          # > L2 (126 MB) write between timed launches
+                flush.zero_()          # > L2 (50 MB) write between timed launches
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
             fn()
@@ -133,7 +121,7 @@ def kernel_probes(tts, cfg, n_mel, B, P, iters=200):
     ms = timeit(lambda: lib.gemm(a, w, M=S, N=C, K=C, taps=3, pad=1, bias=bb, residual=x, out_f32=x, batch=2, a_bstride=S * C,
                                  res_bstride=S * C, outf_bstride=S * C), flush=flush)
     flops = 2 * 2.0 * S * C * 3 * C
-    out.append(dict(kernel="diffusion conv k=3 GEMM (tcgen05, M=2x%d N=1024 K=3072)" % S, bound="tensor", ms=ms,
+    out.append(dict(kernel="diffusion conv k=3 GEMM (wgmma, M=2x%d N=1024 K=3072)" % S, bound="tensor", ms=ms,
                     count=16 * iters, achieved=flops / ms / 1e9, peak=tfl, unit="TFLOP/s"))
     # (3) the AR decode step at the mean context (step n_mel/2): ONE kernel = all 30 layers + mel_head for every candidate
     # of this GPU. Algorithmic bytes per launch (DESIGN §4): every weight once (bf16) + the shared prompt K/V once per layer
@@ -159,7 +147,7 @@ def kernel_probes(tts, cfg, n_mel, B, P, iters=200):
                         bound="hbm", ms=ms, count=(n_mel - 1) if mode == "fused" else 0,
                         achieved=(w_bytes + kv_bytes) / ms / 1e6, peak=hbm, unit="GB/s", algorithmic_bytes=w_bytes + kv_bytes))
         # the attention kernel as the mixed mode launches it: all L layers back to back (every layer streams its own
-        # slice of the 13.5 GB cache, so nothing is reused from the 126 MB L2 between launches), per-launch = / L
+        # slice of the KV cache, so nothing is reused from the 50 MB L2 between launches), per-launch = / L
         def all_layers():
             for l in range(L):
                 hd.step(phase_mask=4, layer_begin=l, layer_end=l + 1)
@@ -287,6 +275,11 @@ def run_engine(args):
         if world > 1:
             dist.destroy_process_group()
         return
+    if args.dump_outputs:
+        # what the caller of the timed path received in the last timed step (same arguments => same seeded inputs)
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "wav.npy"), wav.detach().float().cpu().numpy())
     B = NCAND[preset]
     iters = ITERS[preset]
     h2d = sum(t.numel() * 4 for t in cl_host) * len(utt) + sum(4 * (len(u) + 1) for u in utt)
@@ -308,7 +301,7 @@ def run_engine(args):
         "vs_baseline": None, "dtype": "bf16 tensor-core operands, fp32 accumulate/residual/norm/softmax/scheduler",
         "data": "synthetic (seeded random checkpoint in the reference .pth layout, EOS suppressed; synthetic latents)",
         "config": {"workload": workload,
-                   "l2": "working set (1.9 GB weights + %.1f GB KV cache) >> 126 MB L2; no flush between steps" %
+                   "l2": "working set (1.9 GB weights + %.1f GB KV cache) >> 50 MB L2; no flush between steps" %
                          (2 * 30 * ((B + world - 1) // world if not config5 else B) * 16 * n_mel * 64 * 2 / 1e9),
                    "parallelism": par},
         "e2e": {"value": audio_s / (ms_per_step / 1e3), "unit": UNIT, "h2d_bytes_per_step": h2d,
@@ -327,14 +320,9 @@ def run_engine(args):
         probes, how = kernel_probes(tts, cfg, n_mel, B, len(tokens) + 5, iters)
         progress("probes done")
         dom = max(probes, key=lambda d: d["total_ms_per_utterance"])
-        traffic, source = None, None
-        best = ""
-        for key, val in ncu_traffic().items():          # the most specific (longest) matching probe-name prefix
-            if dom["kernel"].startswith(key) and len(key) > len(best):
-                best, traffic, source = key, val["bytes"], val["source"]
         line["roofline"] = {"kernel": dom["kernel"], "bound": dom["bound"], "achieved": round(dom["achieved"], 2),
-                            "peak": dom["peak"], "unit": dom["unit"], "frac": round(dom["frac"], 4), "traffic": traffic,
-                            "traffic_source": source, "peak_source": how, "launch_ms": round(dom["ms"], 4),
+                            "peak": dom["peak"], "unit": dom["unit"], "frac": round(dom["frac"], 4),
+                            "peak_source": how, "launch_ms": round(dom["ms"], 4),
                             "algorithmic": dom.get("algorithmic_bytes")}
         line["kernels"] = [{k_: (round(v, 4) if isinstance(v, float) else v) for k_, v in d.items()} for d in probes]
         if not args.no_cpu_baseline:
@@ -357,7 +345,7 @@ def _ref_available():
 
 
 def _baseline_cmd(args, device, repeat=1):
-    """The unmodified reference modules when they are importable (oracle/_ref or /root/reference), else the oracle port."""
+    """The unmodified reference modules when they are importable (oracle/_ref), else the oracle port."""
     mod = "oracle.ref_baseline" if _ref_available() else "oracle.cpu_baseline"
     cmd = [sys.executable, "-m", mod, "--preset", args.preset, "--mel-tokens", str(args.mel_tokens),
            "--tokens-json", os.path.join(ROOT, "tests", "golden", "bench_text_tokens.json"), "--text", args.text,
@@ -450,7 +438,11 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-ref-gpu", action="store_true")
     ap.add_argument("--cpu-timeout", type=int, default=240, help="seconds allowed per baseline sample")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the waveform of the last timed step to DIR/wav.npy (float32)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes the engine's output; the reference arm times unit costs and produces no waveform")
     if args.impl == "reference":
         run_reference(args)
     else:

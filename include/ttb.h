@@ -1,4 +1,4 @@
-/* tortoise-b200: C-ABI of the sm_100a kernel library (libttb.so).
+/* tortoise-b200: C-ABI of the sm_90a kernel library (libttb.so).
  *
  * The reference (neonbjb/tortoise-tts) has no FFI layer: its hot path is PyTorch modules calling
  * ATen/cuBLAS/cuDNN. This header is the boundary a maintainer would bind instead (ctypes stub in
@@ -20,10 +20,10 @@ extern "C" {
 
 const char* ttb_last_error(void);
 int ttb_version(void);
-/* 1 if the current device is compute capability 10.x (the only supported target), else 0 */
+/* 1 if the current device is compute capability 9.0 (sm_90a, the only supported target), else 0 */
 int ttb_device_ok(void);
 
-/* ---------------------------------------------------------------- dense contraction (tcgen05) */
+/* ---------------------------------------------------------------- dense contraction (wgmma) */
 enum { TTB_ACT_NONE = 0, TTB_ACT_GELU_NEW = 1, TTB_ACT_SILU = 2, TTB_ACT_GEGLU = 3, TTB_ACT_LRELU02 = 4, TTB_ACT_TANH = 5 };
 
 typedef struct TtbGemmArgs {
@@ -50,7 +50,7 @@ typedef struct TtbGemmArgs {
   int variant;          /* 0 = auto; 1 = one tile per CTA; 2 = persistent kernel; with tile_n = 32 also 3 / 4 = one tile
                            per CTA with a 5- / 4-stage pipeline (tools/gemm_sweep.py, tools/gemm_diag.py).
                            Experiments not yet validated on hardware (never chosen automatically): 5 = two TMA issuer
-                           threads per CTA, 6 = CTA-pair kernel (tcgen05 cta_group::2, 256 x tile_n tiles, tile_n 128 / 256) */
+                           threads per CTA, 6 = reserved (rejected) */
   float* gn_partials;   /* non-NULL: the epilogue also leaves the GroupNorm statistics of its OUTPUT (after bias, activation
                            and residual) in a ttb_groupnorm scratch buffer: (sum, sum of squares) of every 32-row x 32-column
                            block, i.e. one partial per (batch item, group, row block) for 32 channels per group. Needs
@@ -63,7 +63,7 @@ typedef struct TtbGemmArgs {
                            dependent launch); results do not change */
 } TtbGemmArgs;
 
-/* nn.Linear / HF Conv1D / nn.Conv1d(k=1,3) as one tcgen05 GEMM with fused bias/activation/residual.
+/* nn.Linear / HF Conv1D / nn.Conv1d(k=1,3) as one wgmma GEMM with fused bias/activation/residual.
  * Replaces: GPT2 c_attn/c_proj/c_fc (HF 4.31 modeling_gpt2, via models/autoregressive.py:150-163),
  * mel_head (autoregressive.py:42), CLVP to_q/k/v/to_out/FF (models/xtransformers.py:519-521,429-474),
  * DiffusionTts convs (models/diffusion_decoder.py:83-103, models/arch_util.py:107-111),
@@ -126,7 +126,7 @@ typedef struct TtbAttnArgs {
   float* lse;           /* fp32 [nseq*T, H], log2 domain, or NULL */
   int bias_sat;         /* > 0: bias[h][r] == bias[h][-(T-1)] for r <= -bias_sat and == bias[h][T-1] for r >= bias_sat
                            (T5 buckets saturate at max_distance); lets far-from-diagonal tiles skip the table. 0 = unknown */
-  int head_dim;         /* 0 or 64: heads of 64 (tcgen05 kernels). 32 / 96 / 128: short sequences, packed form only; head h
+  int head_dim;         /* 0 or 64: heads of 64 (wgmma kernels). 32 / 96 / 128: short sequences, packed form only; head h
                            at column head_dim * h (diffusion contextual embedder: 2048 channels / 16 heads) */
 } TtbAttnArgs;
 /* softmax(q k^T * scale + bias) v per (sequence, head), head_dim 64. Replaces QKVAttentionLegacy

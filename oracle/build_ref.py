@@ -1,10 +1,10 @@
-"""TEST/BENCH INFRASTRUCTURE ONLY — makes the UNMODIFIED reference importable on the GPU box.
+"""TEST/BENCH INFRASTRUCTURE ONLY — makes the UNMODIFIED reference importable from inside the repository tree.
 
 The reference (neonbjb/tortoise-tts) is pure Python: "building" it is copying its package where the shims
-(oracle/ref_shims.py) can import it. /root/reference exists only in the build container; this recipe copies
+(oracle/ref_shims.py) can import it. Where a checkout of the reference exists (TORTOISE_REFERENCE_ROOT), this recipe copies
 `tortoise/` (sources + the small data assets + three voice clips used by BASELINE configs[1]) to `oracle/_ref/tortoise`,
-which is git-ignored (the sources never enter this repository's history) but travels to the GPU box with the snapshot,
-like a built .so. `__graft_entry__.build()` runs it whenever /root/reference is present.
+which is git-ignored (the sources never enter this repository's history) but travels with a copy of the built tree,
+like a built .so. `__graft_entry__.build()` runs it whenever the checkout is present.
 
   python -m oracle.build_ref
 """
@@ -19,7 +19,7 @@ KEEP_VOICES = ("angie", "cond_latent_example")
 def build(force=False):
     src = os.path.join(SRC, "tortoise")
     if not os.path.isdir(src):
-        return None                                  # GPU box: use what the snapshot brought
+        return None                                  # no checkout here: use the copy made earlier, if any
     dst = os.path.join(DST, "tortoise")
     stamp = os.path.join(DST, ".stamp")
     want = str(sorted((os.path.relpath(os.path.join(d, f), src), os.path.getsize(os.path.join(d, f)))

@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE ONLY — loader for the unmodified reference (neonbjb/tortoise-tts).
 
-Imports the reference's own PyTorch modules from /root/reference (present only in the
-build container, never on the GPU box) so that (a) oracle/*.py restatements can be
+Imports the reference's own PyTorch modules from a checkout of the reference (TORTOISE_REFERENCE_ROOT) or, where
+there is none, from the copy that oracle/build_ref.py placed under oracle/_ref, so that (a) oracle/*.py restatements can be
 validated against them and (b) golden vectors under tests/golden/ can be generated
 (tests/golden/make_golden.py).  Nothing in the product path may import this file.
 
@@ -15,7 +15,7 @@ import types
 _VENDORED = os.path.join(os.path.dirname(os.path.abspath(__file__)), "_ref")    # oracle/build_ref.py (git-ignored copy)
 REFERENCE_ROOT = os.environ.get("TORTOISE_REFERENCE_ROOT", "/root/reference")
 if not os.path.isdir(os.path.join(REFERENCE_ROOT, "tortoise")) and os.path.isdir(os.path.join(_VENDORED, "tortoise")):
-    REFERENCE_ROOT = _VENDORED                # GPU box: the unmodified reference package as copied by the build recipe
+    REFERENCE_ROOT = _VENDORED                # the unmodified reference package as copied by the build recipe
 
 
 def reference_available() -> bool:

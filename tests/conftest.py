@@ -9,8 +9,8 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
-    config.addinivalue_line("markers", "reference: needs /root/reference (build container only)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
+    config.addinivalue_line("markers", "reference: needs the reference package that build() places under oracle/_ref")
 
 
 def pytest_collection_modifyitems(config, items):

@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """CPU study (not a test): error of ONE denoiser evaluation (eps/variance prediction, both CFG branches) when the
 conv / attention GEMM operands are rounded to bf16 (the engine today) or to FP8 e4m3 (per-tensor scale for weights,
-per-token scale for activations). FP8 operands would halve the bytes the TMA has to deliver per k-block, which is what
-bounds the tcgen05 GEMM today (DESIGN.md §9 item 1); the parity bound on this check is 3 %.
+per-token scale for activations). FP8 operands would halve the bytes the TMA has to deliver per k-block;
+the parity bound on this check is 3 %.
 Run: python tests/study_gemm_precision.py"""
 import os
 import sys

@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 GEMM / conv-as-GEMM (ttb_gemm) against a plain PyTorch fp32 reference of the same op on the
+"""GPU: the wgmma GEMM / conv-as-GEMM (ttb_gemm) against a plain PyTorch fp32 reference of the same op on the
 same bf16-rounded operands (tolerance: fp32 accumulation-order noise, 2e-3 relative to the output scale), and the
 SIMT checker kernel against the same reference."""
 import pytest
@@ -170,17 +170,11 @@ def test_gemm_simt_checker(case):
 
 EXPERIMENTAL = [
     dict(M=1872, N=1024, K=1024, taps=3, batch=2, residual=True, tile_n=128, variant=5),   # two TMA issuer threads
-    dict(M=256, N=256, K=128, tile_n=256, variant=6),                                       # CTA pair, one tile
-    dict(M=300, N=512, K=256, tile_n=128, variant=6, act=1, out="both"),                   # CTA pair, M tail, 128-wide
-    dict(M=1872, N=1024, K=1024, taps=3, batch=2, residual=True, tile_n=256, variant=6),   # CTA pair, conv k=3 shape
-    dict(M=3000, N=2304, K=768, out="bf16", tile_n=256, variant=6),                         # CTA pair, CLVP qkv shape
 ]
 
 
 @pytest.mark.skipif(__import__("os").environ.get("TTB_TEST_EXPERIMENTAL") != "1",
-                    reason="GEMM variants 5 / 6 (two TMA issuers, CTA pair) are not on the product path (they ran correctly on "
-                           "B200 in round 2 and lost to the default kernel, profiles/gemm_sweep_r02_with_2cta.txt): opt in with "
-                           "TTB_TEST_EXPERIMENTAL=1")
+                    reason="GEMM variant 5 (two TMA issuers) is not on the product path: opt in with TTB_TEST_EXPERIMENTAL=1")
 @pytest.mark.parametrize("case", EXPERIMENTAL, ids=[str(i) for i in range(len(EXPERIMENTAL))])
 def test_gemm_experimental_variants(case):
     y, of, ob = _run(**case)

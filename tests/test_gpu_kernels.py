@@ -9,6 +9,14 @@ from gpu_util import report
 pytestmark = pytest.mark.gpu
 
 
+def test_device_ok():
+    """The library accepts the device it is compiled for (compute capability 9.0)."""
+    from tortoise_tts_b200 import lib
+    torch.cuda.init()
+    assert torch.cuda.get_device_capability() == (9, 0)
+    assert lib.load().ttb_device_ok() == 1
+
+
 def test_layernorm_single_and_chained():
     from tortoise_tts_b200 import lib
     torch.manual_seed(0)
@@ -156,7 +164,7 @@ def test_attention(T, H, nseq, causal, use_bias):
     from tortoise_tts_b200.diffusion_engine import _rel_pos_table
     torch.manual_seed(3)
     D = H * 64
-    # "big": scores spanning > 2^8 so that the lazy O rescale in TMEM is exercised
+    # "big": scores spanning > 2^8 so that the lazy O rescale is exercised
     qkv = (torch.randn(nseq * T, 3 * D, device="cuda") * (4.0 if use_bias == "big" else 1.0)).to(torch.bfloat16)
     sat = 0
     if use_bias == "t5":      # saturated T5 relative-position table (fast-tile path of the flash kernel)

@@ -154,7 +154,7 @@ def test_sampled_mel_200_steps(full):
     steps (where both still see the same x): |dx| after step 1 <= 3 % of |x|; and distributional on the final mel
     (gpu_util.check_sampled_mel: rms <= 0.3, 99.9th percentile <= 1.5 of the 13.8 mel range = 1.5 x the drift measured
     when the fp32 oracle itself is run with bf16-rounded GEMM operands, tests/test_host_orchestration.py; max <= 4.0). The full per-step max / rms series goes to the
-    parity log (gpurun_out/errors.jsonl -> profiles/parity_errors_r02.jsonl)."""
+    parity log (gpu_util.report)."""
     from tortoise_tts_b200.synth import synth_diffusion
     from tortoise_tts_b200.diffusion_engine import DiffusionEngine
     from oracle import diffusion as od

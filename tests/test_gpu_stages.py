@@ -2,8 +2,8 @@
 the committed golden vectors generated from the reference modules.
 
 Tolerances (stated per test): GEMM operands are bf16 with fp32 accumulation, the residual stream / norms / softmax
-statistics / scheduler are fp32; the reference is fp32 end-to-end.  Bounds below are ~3x the measured error on B200
-(see profiles/parity_r01.md) and are relative to the natural scale of each quantity.
+statistics / scheduler are fp32; the reference is fp32 end-to-end.  Bounds below are ~3x the measured error
+and are relative to the natural scale of each quantity.
 """
 import os
 

@@ -1,6 +1,5 @@
-"""Pins oracle/*.py against the UNMODIFIED reference modules (build container only; the
-reference tree does not travel to the GPU box, where these tests skip and the committed
-tests/golden/* fixtures carry the pin instead)."""
+"""Pins oracle/*.py against the UNMODIFIED reference modules (the copy build() places under oracle/_ref; without
+it these tests skip and the committed tests/golden/* fixtures carry the pin instead)."""
 import os
 
 import numpy as np

@@ -1,5 +1,5 @@
 """Long-form text splitter (tortoise_tts_b200/text.py) against the reference's own known-answer tests, committed
-reference outputs on seeded synthetic texts, and (where /root/reference exists) the reference function itself."""
+reference outputs on seeded synthetic texts, and (where build() has placed the reference under oracle/_ref) the reference function itself."""
 import importlib.util
 import json
 import os
@@ -67,9 +67,8 @@ def test_utterance_plan():
 
 @pytest.mark.reference
 def test_against_reference_function():
-    path = "/root/reference/tortoise/utils/text.py"
-    if not os.path.exists(path):
-        pytest.skip("reference tree not present")
+    from oracle.ref_shims import REFERENCE_ROOT
+    path = os.path.join(REFERENCE_ROOT, "tortoise", "utils", "text.py")
     spec = importlib.util.spec_from_file_location("ref_text", path)
     ref = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(ref)

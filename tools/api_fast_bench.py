@@ -1,4 +1,4 @@
-"""Times the `api_fast` path (SURVEY 8f row 3) at full size on one B200: `tts()` (one sequence -> latents -> HiFiGAN)
+"""Times the `api_fast` path (SURVEY 8f row 3) at full size on one H100: `tts()` (one sequence -> latents -> HiFiGAN)
 and `tts_stream()` (first-chunk latency, total). Synthetic checkpoint with the stop token suppressed, so `tts()` runs
 the model's 603-token limit and the stream runs `500 - prompt` tokens (autoregressive.py:553,571). Prints one JSON line.
 The reference publishes, for this path only, "RTF 0.25-0.3" and "< 500 ms" to the first chunk on an unnamed GPU

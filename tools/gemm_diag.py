@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Where does the tcgen05 GEMM spend its time?
+"""Where does the wgmma GEMM spend its time?
  (1) per-launch time of back-to-back launches (host latency amortised, warm L2) next to torch.matmul (cuBLAS);
  (2) per-CTA phase timestamps (ttb_debug_gemm_trace): setup, first operand latency, mainloop, drain, epilogue, and
      how many CTAs an SM really runs at a time.
@@ -42,16 +42,16 @@ def trace(lib, fn, ctas, label):
     t0 = t[:, 0].min()
     span = (t[:, 7].max() - t0).item()
     ph = {
-        "setup (alloc, barriers)": t[:, 2] - t[:, 0],
-        "first operands landed": t[:, 3] - t[:, 2],
-        "mainloop issue": t[:, 4] - t[:, 3],
-        "drain to accum ready": t[:, 5] - t[:, 4],
+        "setup (barriers, dependency wait)": t[:, 2] - t[:, 0],
+        "consumers reach the main loop": t[:, 3] - t[:, 2],
+        "main loop (wgmma retired)": t[:, 4] - t[:, 3],
+        "accumulator staged": t[:, 5] - t[:, 4],
         "epilogue": t[:, 6] - t[:, 5],
-        "tail (dealloc)": t[:, 7] - t[:, 6],
+        "tail": t[:, 7] - t[:, 6],
         "CTA lifetime": t[:, 7] - t[:, 0],
     }
-    print("-- trace %s: %d CTAs, kernel span %.1f us, sum(lifetime)/(span*148) = %.2f CTAs resident per SM on average"
-          % (label, ctas, span / 1e3, (ph["CTA lifetime"].sum().item() / (span * 148))))
+    print("-- trace %s: %d CTAs, kernel span %.1f us, sum(lifetime)/(span*SMs) = %.2f CTAs resident per SM on average"
+          % (label, ctas, span / 1e3, (ph["CTA lifetime"].sum().item() / (span * torch.cuda.get_device_properties(0).multi_processor_count))))
     for k, v in ph.items():
         print("   %-26s mean %7.2f us   p10 %7.2f   p90 %7.2f" % (k, v.mean().item() / 1e3, v.quantile(0.1).item() / 1e3,
                                                                     v.quantile(0.9).item() / 1e3))

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Times the tcgen05 GEMM variants (tile width, one-tile-per-CTA vs persistent, cluster multicast, split-K) on the
+"""Times the wgmma GEMM variants (tile width, one-tile-per-CTA vs persistent, cluster multicast, split-K) on the
 shapes of the hot path, next to torch.matmul (cuBLAS) as a calibration of what the hardware delivers on that shape.
 Development aid; prints a table. L2 is flushed between timed launches."""
 import os
@@ -73,8 +73,7 @@ def main():
                 if tile != 256 and ((N + tile - 1) // tile) % cl == 0:
                     variants.append(dict(tile_n=tile, cluster=cl))
         if os.environ.get("TTB_TEST_EXPERIMENTAL") == "1" and M > 256:
-            # round-2 kernels, not yet run on hardware (run the sweep under `timeout`): two TMA issuers, CTA pairs
-            variants += [dict(tile_n=128, variant=5), dict(tile_n=128, variant=6), dict(tile_n=256, variant=6)]
+            variants += [dict(tile_n=128, variant=5)]          # two TMA issuer threads
         if name == "ar proj2":
             variants = [dict(tile_n=t, splitk=s, cluster=c) for t in (32, 64, 128) for s in (2, 4, 8) for c in (0, 4)
                         if c == 0 or ((N + t - 1) // t) % c == 0]

@@ -1,4 +1,4 @@
-"""Drop-in facade for `tortoise.api.TextToSpeech` (tortoise/api.py:174-609) on the sm_100a engine.
+"""Drop-in facade for `tortoise.api.TextToSpeech` (tortoise/api.py:174-609) on the sm_90a engine.
 
 Same constructor / `tts()` / `tts_with_preset()` signatures, presets, return types and checkpoint layout
 (`models_dir` with autoregressive.pth, diffusion_decoder.pth, clvp2.pth, vocoder.pth). Everything between the
@@ -198,7 +198,7 @@ class TextToSpeech:
         """`state_dicts` (dict with keys autoregressive/diffusion/clvp/vocoder) bypasses models_dir (synthetic
         checkpoints); `config` overrides the full-size ModelConfig (tests)."""
         if not torch.cuda.is_available():
-            raise RuntimeError("tortoise_tts_b200 needs a CUDA device (sm_100a); there is no CPU path")
+            raise RuntimeError("tortoise_tts_b200 needs a CUDA device (sm_90a); there is no CPU path")
         lib.load()
         self.models_dir = models_dir
         self.autoregressive_batch_size = autoregressive_batch_size  # accepted for API parity; one batch is used

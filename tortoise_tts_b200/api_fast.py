@@ -1,4 +1,4 @@
-"""Drop-in facade for `tortoise.api_fast.TextToSpeech` (tortoise/api_fast.py:171-520) on the sm_100a engine: the
+"""Drop-in facade for `tortoise.api_fast.TextToSpeech` (tortoise/api_fast.py:171-520) on the sm_90a engine: the
 reference's low-latency product path — ONE autoregressive sequence, no CLVP / diffusion, GPT latents rendered
 directly by the HiFiGAN decoder (`hifidecoder.pth`), optionally streamed chunk by chunk.
 
@@ -58,7 +58,7 @@ class TextToSpeech:
         """`state_dicts` (keys autoregressive / hifigan [/ rlg_auto / mel_norms]) bypasses models_dir (synthetic
         checkpoints); `config` overrides the full-size ModelConfig (tests)."""
         if not torch.cuda.is_available():
-            raise RuntimeError("tortoise_tts_b200 needs a CUDA device (sm_100a); there is no CPU path")
+            raise RuntimeError("tortoise_tts_b200 needs a CUDA device (sm_90a); there is no CPU path")
         lib.load()
         self.models_dir = models_dir
         self.autoregressive_batch_size = autoregressive_batch_size     # accepted for API parity (one sequence is decoded)

@@ -1,4 +1,4 @@
-"""UnifiedVoice autoregressive stage on the sm_100a kernels (hot loop 1 + latents, SURVEY §8 rows a1-a4, a7).
+"""UnifiedVoice autoregressive stage on the sm_90a kernels (hot loop 1 + latents, SURVEY §8 rows a1-a4, a7).
 
 Host side mirrors `UnifiedVoice.inference_speech` / `UnifiedVoice.forward(return_latent=True)`
 (tortoise/models/autoregressive.py:535-563, 454-512): same inputs (conditioning latent, zero-padded text
@@ -58,17 +58,15 @@ class AREngine:
     DECODE_CLUSTER = int(_os.environ.get("TTB_AR_CLUSTER", "0"))
     # TTB_AR_WIDE=1: c_attn / c_fc (N = 3D, 4D: one wave of 64-wide tiles) use 64-column tiles with an 8-stage pipeline
     DECODE_WIDE = int(_os.environ.get("TTB_AR_WIDE", "0"))
-    # TTB_AR_FUSED=1 (default): the decode step is ONE persistent kernel (csrc/ar_step.cu) + the sampler; 0 = the round-1
+    # TTB_AR_FUSED=1 (default): the decode step is ONE persistent kernel (csrc/ar_step.cu) + the sampler; 0 = the
     # per-op CUDA graph (kept as the A/B baseline and for shapes the fused kernel does not cover)
     FUSED = int(_os.environ.get("TTB_AR_FUSED", "1"))
-    # How the step runs when the one-kernel form is available (measured on B200, tools/ar_step_probe.py, step time at
-    # context 174+215): "fused" = everything in the persistent kernel: 1.85 ms at 32 candidates (per-op graph: 2.28), but
-    # its phases grow with the batch (2.8 / 3.7 / 4.1 ms at 64 / 128 / 256 against 2.2 / 2.4 / 3.1): one CTA per SM
-    # serialises TMA wait -> MMA -> epilogue inside a phase, which several small kernels per SM overlap. "mixed" = the
-    # per-op graph with its three attention kernels (prefix flash + candidate stream + merge, 65 us at 256 candidates)
-    # replaced by the persistent kernel's attention phase (one launch, 54 us). "auto" picks by batch size. End of round 2
-    # (PDL with tail / early triggers, the tensor-core attention kernel): the mixed step also wins at 32 candidates (AR 690
-    # against 847 ms for 429 steps), so the one-kernel step is kept for small batches only (one sequence: 1.59 ms / token).
+    # How the step runs when the one-kernel form is available: "fused" = everything in the persistent kernel, whose
+    # phases grow with the batch (one CTA per SM serialises TMA wait -> MMA -> epilogue inside a phase, which several
+    # small kernels per SM overlap). "mixed" = the per-op graph with its three attention kernels (prefix flash + candidate
+    # stream + merge) replaced by the persistent kernel's attention phase (one launch). "auto" picks by batch size: the
+    # one-kernel step for small batches only (H100 80GB HBM3, 700 W, 256 candidates, 429 steps: AR 1.73 s mixed against
+    # 3.50 s fused; the batch size where the two cross, FUSED_MAX_B, has not been measured on H100).
     MODE = _os.environ.get("TTB_AR_MODE", "auto")            # auto | fused | mixed | perop
     FUSED_MAX_B = int(_os.environ.get("TTB_AR_FUSED_MAX_B", "16"))
     # TTB_AR_CHAINS=2: in mixed mode the candidates are decoded as TWO independent half-batches on two streams inside
@@ -78,7 +76,10 @@ class AREngine:
     # which decode GEMMs may fetch their weights ahead of griddepcontrol.wait (TtbGemmArgs.w_static): "ln" = the ones that
     # follow a LayerNorm (which triggers its dependents early), "all", "none"
     WSTATIC = _os.environ.get("TTB_AR_WSTATIC", "ln")
-    CHAINS = int(_os.environ.get("TTB_AR_CHAINS", "2"))     # measured: AR 1157 -> 1092 ms at 256 candidates, 860 -> 840 at 128
+    # measured on H100 (80GB HBM3, 700 W) at 256 candidates: AR 1839 ms with one chain, 1727 ms with two; split-K 2 / 4
+    # against none: 1727 against 1795 ms; weight prefetch ahead of the dependency wait ("ln" against "none"): 1727 / 1731 ms
+    # (inside the run-to-run spread). CHAINS_MIN_B has not been measured on H100.
+    CHAINS = int(_os.environ.get("TTB_AR_CHAINS", "2"))
     CHAINS_MIN_B = int(_os.environ.get("TTB_AR_CHAINS_MIN_B", "128"))
     SPLITK_PROJ = int(_os.environ.get("TTB_AR_SPLITK_PROJ", "2"))     # attn.c_proj (K = D): 32 n-tiles x 2 m-tiles x 2 splits = 128 CTAs at D=1024, B=256
     SPLITK_PROJ2 = int(_os.environ.get("TTB_AR_SPLITK_PROJ2", "4"))   # mlp.c_proj (K = 4D): 32 x 2 x 4 = 256 CTAs

@@ -1,4 +1,4 @@
-"""Builds libttb.so (the sm_100a kernel library behind include/ttb.h) in-tree with nvcc."""
+"""Builds libttb.so (the sm_90a kernel library behind include/ttb.h) in-tree with nvcc."""
 import hashlib
 import os
 import subprocess
@@ -8,14 +8,14 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libttb.so")
 STAMP = LIB + ".stamp"      # content hash of the sources the library was built from (travels with the .so)
-SOURCES = ["capi.cu", "gemm.cu", "norm.cu", "attention.cu", "flash_attn.cu", "flash_attn2.cu", "ar.cu", "ar_step.cu", "misc.cu", "vocoder.cu", "audio.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "--use_fast_math",
+SOURCES = ["capi.cu", "gemm.cu", "norm.cu", "attention.cu", "flash_attn.cu", "ar.cu", "ar_step.cu", "misc.cu", "vocoder.cu", "audio.cu"]
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "--use_fast_math",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-O3"]
 
 
 def _source_hash():
     """Hash of every file under csrc/ + the public header + the flags. File times are not used: a copy of the tree
-    (the GPU box receives one) need not preserve them, and a spurious rebuild costs minutes there."""
+    need not preserve them, and a spurious rebuild costs minutes."""
     h = hashlib.sha256(" ".join(NVCC_FLAGS).encode())
     files = [os.path.join(CSRC, f) for f in sorted(os.listdir(CSRC))] + [os.path.join(HERE, "..", "include", "ttb.h")]
     for f in files:
@@ -48,7 +48,7 @@ def build(force=False, verbose=False):
         raise RuntimeError("nvcc failed")
     cmd = [nvcc, "-shared", "-o", LIB + ".tmp"] + objs + ["-lcudart"]
     subprocess.check_call(cmd)
-    os.replace(LIB + ".tmp", LIB)          # atomic: a concurrent reader (repo snapshot) sees the old or the new library
+    os.replace(LIB + ".tmp", LIB)          # atomic: a concurrent reader sees the old or the new library
     with open(STAMP + ".tmp", "w") as f:
         f.write(want + "\n")
     os.replace(STAMP + ".tmp", STAMP)

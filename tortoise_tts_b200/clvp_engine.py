@@ -1,4 +1,4 @@
-"""CLVP re-ranker on the sm_100a kernels (SURVEY §8 row a5).
+"""CLVP re-ranker on the sm_90a kernels (SURVEY §8 row a5).
 
 Mirrors `CLVP.forward(text, speech_tokens, return_loss=False)` (tortoise/models/clvp.py:99-140) for the
 x-transformers Encoder configuration the reference builds (clvp.py:54-83). The text latent is computed ONCE per

@@ -1,4 +1,4 @@
-"""Conditioning front-end on the sm_100a kernels (SURVEY §8f-1): reference clips -> (auto latent [1, D], diffusion latent
+"""Conditioning front-end on the sm_90a kernels (SURVEY §8f-1): reference clips -> (auto latent [1, D], diffusion latent
 [1, 2C]).
 
 Mirrors `TextToSpeech.get_conditioning_latents` (tortoise/api.py:258-299):

@@ -1,16 +1,16 @@
-// One GPT-2 decode step of the UnifiedVoice sampler as ONE persistent kernel (sm_100a).
+// One GPT-2 decode step of the UnifiedVoice sampler as ONE persistent kernel (sm_90a).
 //
 // Replaces, per generated token, GPT2InferenceModel.forward (models/autoregressive.py:108-186) + the 30 HF GPT2Block
-// forwards behind it + final_norm + mel_head for ALL candidates of the batch. Round 1 ran this as a CUDA graph of ~275
-// kernels (LN, 4 skinny GEMMs, 3 attention kernels per layer); the launch chain, not bytes or flops, bounded the step
-// (3.07 ms at 256 candidates, 2.28 ms at 32). Here the whole step is one cooperative launch of one CTA per SM that walks
+// forwards behind it + final_norm + mel_head for ALL candidates of the batch. As a CUDA graph of ~275
+// kernels (LN, 4 skinny GEMMs, 3 attention kernels per layer) the launch chain, not bytes or flops, bounds the step.
+// Here the whole step is one cooperative launch of one CTA per SM that walks
 // the layer phases with grid-wide barriers:
 //
 //   embed + ln_1 | for each layer: QKV GEMM | attention (+KV append) | c_proj GEMM | residual + ln_2 | c_fc GEMM + gelu_new
 //                |                 mlp.c_proj GEMM | residual + next ln_1 (or ln_f -> final_norm) | ... | mel_head GEMM
 //
-// GEMM phases ("swap-AB" skinny GEMM): the WEIGHT rows are the UMMA M dimension (128-row tiles streamed once from HBM by
-// TMA) and the candidate batch is the UMMA N dimension (16..128 columns), so a 32-candidate step does not pay for a
+// GEMM phases ("swap-AB" skinny GEMM): the WEIGHT rows are the wgmma M dimension (128-row tiles streamed once from HBM by
+// TMA, 64 rows per consumer warpgroup) and the candidate batch is the wgmma N dimension (16..128 columns), so a 32-candidate step does not pay for a
 // 128-row activation tile. Work items = (row tile, batch tile, K split); split-K partials are reduced in a fixed order
 // by the last CTA to finish a tile (ticket counter), which also applies bias / gelu_new and writes the bf16 result, or
 // - for the two GEMMs that feed the residual stream - by the LayerNorm phase that follows.
@@ -58,7 +58,7 @@ struct AsLayer {       // device table, one per layer
 
 struct AsParams {
   int B, D, H, L, V, P, Nmax, pos_mode;
-  int TB, nbt, nst, stage_bytes;          // batch tile (UMMA N), number of batch tiles, pipeline stages
+  int TB, nbt, nst, stage_bytes;          // batch tile (wgmma N), number of batch tiles, pipeline stages
   int ncph, ipr, team;                    // attention: CTAs per head, items per round, warps per item
   int prefetch;
   int sync_mode;                          // grid barrier flavour (TTB_AR_STEP_SYNC): 0 = conservative, 1 = light
@@ -149,10 +149,8 @@ TTB_DEVINL void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0
 struct AsCtrl {                       // lives in the control block of shared memory
   uint64_t full_bar[AS_MAX_STAGES];
   uint64_t empty_bar[AS_MAX_STAGES];
-  uint64_t acc_full, acc_empty;
   uint64_t ring_bar[AS_WARPS][4];
   uint64_t prefix_bar;
-  uint32_t tmem_slot;
   uint32_t ticket;
   float red[4][AS_WARPS];
   float merge[AS_WARPS][68];          // flash-decoding merge: acc[64], m, l
@@ -167,17 +165,16 @@ struct AsCtrlCompact {                // control block of ar_attn_compact_kernel
 constexpr int AS_CTRL_COMPACT_BYTES = (int)((sizeof(AsCtrlCompact) + 127) & ~size_t(127));
 
 struct AsRole {                       // per-thread pipeline bookkeeping that survives across phases
-  int stage;                          // GEMM smem ring position (producer and MMA thread keep identical copies)
+  int stage;                          // GEMM smem ring position (producer and consumer threads keep identical copies)
   uint32_t phase;
-  uint32_t acc_par;                   // accumulator full/empty parity (MMA thread and epilogue threads)
   uint32_t ring_par[4];               // attention ring parities of this warp
   uint32_t prefix_par;
   unsigned long long bar_target;      // next grid-barrier target
 };
 
 // ------------------------------------------------------------------ grid-wide barrier
-// Arrivals are spread over AS_BAR_SLOTS counters, each on its own 128-byte line: 148 same-address atomics serialise in one
-// L2 slice (~1 us of the 1.7 us the single-counter barrier cost); the first AS_BAR_SLOTS lanes of warp 0 poll one
+// Arrivals are spread over AS_BAR_SLOTS counters, each on its own 128-byte line: one atomic per CTA on the same address serialises in one
+// L2 slice; the first AS_BAR_SLOTS lanes of warp 0 poll one
 // counter each. Counters are monotonic: slot k ends barrier number E at E * (number of CTAs mapped to slot k).
 constexpr int AS_BAR_SLOTS = 16;
 constexpr int AS_BAR_STRIDE = 16;          // u64 elements between slots (128 bytes)
@@ -244,8 +241,7 @@ TTB_DEVINL void prefetch_gemm_item(const AsParams& p, const CUtensorMap* mw, con
 // out[b, n] = act( sum_k act_in[b, k] * W[n, k] + bias[n] ),  n in [0, Nrows), b in [0, B)
 template <int OUT, int ACT>
 TTB_DEVINL void gemm_phase(const AsParams& p, const AsGemmShape& g, const CUtensorMap* mw, const CUtensorMap* ma,
-                           const float* __restrict__ bias, void* out, int ldo, uint8_t* data, AsCtrl* ctrl, AsRole& rl,
-                           uint32_t tmem_base) {
+                           const float* __restrict__ bias, void* out, int ldo, uint8_t* data, AsCtrl* ctrl, AsRole& rl) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   int* err = &p.state->reserved[0];
   const int TB = p.TB;
@@ -269,62 +265,61 @@ TTB_DEVINL void gemm_phase(const AsParams& p, const AsGemmShape& g, const CUtens
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    if (lane == 0) {
-      const uint32_t idesc = umma_idesc_bf16(128, TB, 0, 0);
-      for (int item = blockIdx.x; item < g.items; item += gridDim.x) {
-        const int ks = item % g.nsplit;
-        const int kb0 = ks * g.kbps;
-        const int nkb = min(g.kbps, g.KB - kb0);
-        mbar_wait_to(&ctrl->acc_empty, rl.acc_par ^ 1, err);     // epilogue has drained the previous accumulator
-        tc_fence_after();
-        for (int i = 0; i < nkb; ++i) {
-          mbar_wait_to(&ctrl->full_bar[rl.stage], rl.phase, err);
-          tc_fence_after();
-          const uint32_t sw = smem_u32(data + rl.stage * p.stage_bytes);
-          const uint32_t sa = sw + AS_W_TILE_BYTES;
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            umma_bf16_ss(tmem_base, umma_desc_kmajor_sw128(sw + k * 32), umma_desc_kmajor_sw128(sa + k * 32), idesc,
-                         (i | k) != 0 ? 1u : 0u);
-          umma_commit(&ctrl->empty_bar[rl.stage]);
-          if (++rl.stage == p.nst) { rl.stage = 0; rl.phase ^= 1; }
-        }
-        umma_commit(&ctrl->acc_full);
-        rl.acc_par ^= 1;
-      }
-    }
   } else if (warp >= 4) {
-    // ===== warps 4..7: epilogue (warp w reads TMEM lanes [32 (w % 4), +32) = weight rows; columns = candidates) =====
-    // ===== warps 8..15: idle during the main loop; they join the split-K fix-up of ticketed GEMMs (384 threads) =====
-    const bool epi = warp < 8;
+    // ===== warps 4..7 / 8..11: two consumer warpgroups (weight rows [0, 64) / [64, 128) of the tile; columns =
+    //       candidates): wgmma main loop, then the epilogue straight from the accumulator fragments =====
+    // ===== warps 12..15: idle during the main loop; they join the split-K fix-up of ticketed GEMMs (384 threads) =====
+    const bool epi = warp < 12;
     const bool ticketed = (OUT != OUT_PARTIAL) && g.nsplit > 1;
     if (!epi && !ticketed) return;
-    const int q = warp & 3;
+    const int wg = (warp - 4) >> 2;
+    const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);      // accumulator rows of this thread: row0, row0 + 8
     const int et = threadIdx.x - 128;                  // 0..383 (epilogue threads first)
     for (int item = blockIdx.x; item < g.items; item += gridDim.x) {
       const int ks = item % g.nsplit;
       const int t = item / g.nsplit;
       const int bt = t % p.nbt, rt = t / p.nbt;
-      const int n = rt * 128 + q * 32 + lane;
       const int b_lo = bt * TB;
       if (epi) {
-      mbar_wait_to(&ctrl->acc_full, rl.acc_par, err);
-      rl.acc_par ^= 1;
-      tc_fence_after();
-      const bool direct = (g.nsplit == 1) && (OUT != OUT_PARTIAL);
-      const float bn = (direct && bias && n < g.Nrows) ? __ldg(bias + n) : 0.f;
-      for (int c0 = 0; c0 < TB; c0 += 32) {
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, r);
-        tmem_ld_wait();
-        if (n < g.Nrows) {
+      const int kb0 = ks * g.kbps;
+      const int nkb = min(g.kbps, g.KB - kb0);
+      // the batch tile is TB = 16 nb16 columns wide: one m64n16k16 per 16 candidates (accumulator block j), 8 at most
+      float acc[8][8];
+      int prev = -1;
+      for (int i = 0; i < nkb; ++i) {
+        mbar_wait_to(&ctrl->full_bar[rl.stage], rl.phase, err);
+        const uint32_t sw = smem_u32(data + rl.stage * p.stage_bytes) + wg * (64 * 128);
+        const uint32_t sa = smem_u32(data + rl.stage * p.stage_bytes) + AS_W_TILE_BYTES;
+        wgmma_fence();
 #pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const int b = b_lo + c0 + j;
-            if (c0 + j < TB && b < p.B) {
-              float v = __uint_as_float(r[j]);
+        for (int k = 0; k < 4; ++k) {
+          const uint64_t dw = wgmma_desc_kmajor_sw128(sw + k * 32);
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+            if (j * 16 < TB) wgmma_m64n16k16_bf16_ss(acc[j], dw, wgmma_desc_kmajor_sw128(sa + j * 2048 + k * 32), (i | k) != 0 ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&ctrl->empty_bar[prev]);   // count 2: one arrive per warpgroup
+        prev = rl.stage;
+        if (++rl.stage == p.nst) { rl.stage = 0; rl.phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&ctrl->empty_bar[prev]);
+      const bool direct = (g.nsplit == 1) && (OUT != OUT_PARTIAL);
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int n = rt * 128 + row0 + 8 * hh;
+        if (n >= g.Nrows) continue;
+        const float bn = (direct && bias) ? __ldg(bias + n) : 0.f;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+#pragma unroll
+          for (int r = 0; r < 4; ++r) {
+            const int c = j * 16 + 8 * (r >> 1) + 2 * (lane & 3) + (r & 1);
+            const int b = b_lo + c;
+            if (c < TB && b < p.B) {
+              float v = acc[j][4 * (r >> 1) + 2 * hh + (r & 1)];
               if (direct) {
                 v += bn;
                 if (ACT == TTB_ACT_GELU_NEW) v = gelu_new(v);
@@ -337,9 +332,6 @@ TTB_DEVINL void gemm_phase(const AsParams& p, const AsGemmShape& g, const CUtens
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&ctrl->acc_empty);     // count 4: one arrive per epilogue warp
       }
       if (ticketed) {
         // ticket: the last split to arrive reduces the tile in split order (deterministic), adds bias, activates, writes
@@ -364,7 +356,7 @@ TTB_DEVINL void gemm_phase(const AsParams& p, const AsGemmShape& g, const CUtens
               if (n4 + 3 < g.Nrows) bb.w = __ldg(bias + n4 + 3);
             }
             // 4 rows x all splits in flight per thread before the first add (a dependent chain of L2 round trips
-            // made this fix-up cost 10-25 us per GEMM in the first version)
+            // otherwise dominates this fix-up)
             constexpr int FX_ROWS = 2, FX_SPLITS = 4, FX_LANES = 12;      // 384 threads = 32 column groups x 12 row lanes
             for (int bi0 = (et >> 5); bi0 < nb; bi0 += FX_LANES * FX_ROWS) {
               float4 acc[FX_ROWS];
@@ -611,7 +603,7 @@ TTB_DEVINL void attn_phase(const AsParams& p, int layer, uint8_t* data, AsCtrl* 
 
 // ------------------------------------------------------------------ attention phase, tensor-core form
 // The SIMT form above spends ~14 issue slots per cached position (bf16 unpacking, 8-lane dot products, shuffles): at 256
-// candidates the phase is issue-bound (54 us against 41 us of KV traffic), the shared prompt part alone is 45 % of it.
+// candidates the phase is issue-bound rather than bound by its KV traffic, and the shared prompt part is a large share of it.
 // Here both products of a 16-position chunk run on the tensor cores (mma.sync m16n8k16, bf16 in / fp32 out):
 //   S[16 pos] = K[16 x 64] q      : A = K chunk (row = position), B = q in column 0 of the 16 x 8 operand
 //   O[64]    += V^T[64 x 16] p    : A = V chunk read transposed (ldmatrix.trans), B = p (bf16) in column 0
@@ -788,8 +780,8 @@ TTB_DEVINL void attn_phase_mma(const AsParams& p, int layer, uint8_t* data, Ctrl
         int s = 0;
         // The prompt part (npc chunks already in shared memory, the same for every candidate of this head) is worked
         // off one chunk at a time BEFORE each wait for a candidate tile: the warp would otherwise sit idle at the ring
-        // barrier (a tile takes ~1.7 us to arrive, a chunk ~0.2 us to compute), and doing the prompt part after the
-        // stream left the memory system idle for ~2 us per round.
+        // barrier (a tile takes several times longer to arrive than a chunk takes to compute), and doing the prompt part after
+        // the stream leaves the memory system idle once per round.
         int pc = sub;
         bool prefix_ready = false;
         for (int c_use = sub; c_use < nch; c_use += p.team) {
@@ -818,7 +810,7 @@ TTB_DEVINL void attn_phase_mma(const AsParams& p, int layer, uint8_t* data, Ctrl
         }
         // every stage is free again: start the stream of this warp's NEXT item now, so that its first tiles travel
         // while the prompt part, the merge and the output of this item are computed (the rounds of all warps and SMs
-        // run in step: without this the memory system idles ~6 us per round, tools/dbg/kvstream_probe2.cu)
+        // run in step: without this the memory system idles once per round)
         head_issued = (b + p.ipr < b_end);
         if (head_issued && lane == 0) issue_head(b + p.ipr);
         if (!prefix_ready) mbar_wait_to(&ctrl->prefix_bar, rl.prefix_par, err);
@@ -951,22 +943,16 @@ __global__ void __launch_bounds__(AS_THREADS, 1) ar_step_kernel(const __grid_con
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (warp == 0 && lane == 0) {
-    for (int s = 0; s < AS_MAX_STAGES; ++s) { mbar_init(&ctrl->full_bar[s], 1); mbar_init(&ctrl->empty_bar[s], 1); }
-    mbar_init(&ctrl->acc_full, 1);
-    mbar_init(&ctrl->acc_empty, 4);
+    for (int s = 0; s < AS_MAX_STAGES; ++s) { mbar_init(&ctrl->full_bar[s], 1); mbar_init(&ctrl->empty_bar[s], 2); }
     for (int w = 0; w < AS_WARPS; ++w)
       for (int k = 0; k < 4; ++k) mbar_init(&ctrl->ring_bar[w][k], 1);
     mbar_init(&ctrl->prefix_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<256>(&ctrl->tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = ctrl->tmem_slot;
 
   AsRole rl;
-  rl.stage = 0; rl.phase = 0; rl.acc_par = 0; rl.prefix_par = 0;
+  rl.stage = 0; rl.phase = 0; rl.prefix_par = 0;
   rl.ring_par[0] = rl.ring_par[1] = rl.ring_par[2] = rl.ring_par[3] = 0;
   rl.bar_target = ld_acquire_u64(p.bar);          // barrier epoch at launch (bar[0]; the arrival slots follow)
 
@@ -994,7 +980,7 @@ __global__ void __launch_bounds__(AS_THREADS, 1) ar_step_kernel(const __grid_con
     const CUtensorMap* mw = p.maps + 4 * l;
     if (p.phase_mask & PH_QKV) {
       if (pf) { prefetch_gemm_item(p, mw + G_PROJ, p.g[G_PROJ]); prefetch_gemm_item(p, mw + G_FC, p.g[G_FC]); }
-      gemm_phase<OUT_BF16, TTB_ACT_NONE>(p, p.g[G_QKV], mw + G_QKV, map_a, lw.bqkv, p.qkv, 3 * p.D, data, ctrl, rl, tmem_base);
+      gemm_phase<OUT_BF16, TTB_ACT_NONE>(p, p.g[G_QKV], mw + G_QKV, map_a, lw.bqkv, p.qkv, 3 * p.D, data, ctrl, rl);
       AS_SYNC_UNLESS_LAST(1, l);
     }
     if (p.phase_mask & PH_ATTN) {
@@ -1006,7 +992,7 @@ __global__ void __launch_bounds__(AS_THREADS, 1) ar_step_kernel(const __grid_con
     if (p.phase_mask & PH_NOP) grid_sync(p, rl);
     if (p.phase_mask & PH_PROJ) {
       if (pf) prefetch_gemm_item(p, mw + G_PROJ2, p.g[G_PROJ2]);
-      gemm_phase<OUT_PARTIAL, TTB_ACT_NONE>(p, p.g[G_PROJ], mw + G_PROJ, map_o, nullptr, nullptr, 0, data, ctrl, rl, tmem_base);
+      gemm_phase<OUT_PARTIAL, TTB_ACT_NONE>(p, p.g[G_PROJ], mw + G_PROJ, map_o, nullptr, nullptr, 0, data, ctrl, rl);
       AS_SYNC_UNLESS_LAST(3, l);
     }
     if (p.phase_mask & PH_LN2) {
@@ -1018,11 +1004,11 @@ __global__ void __launch_bounds__(AS_THREADS, 1) ar_step_kernel(const __grid_con
         if (l + 1 < p.L) prefetch_gemm_item(p, mw + 4 + G_QKV, p.g[G_QKV]);
         else prefetch_gemm_item(p, p.maps + 4 * p.L, p.g[G_HEAD]);
       }
-      gemm_phase<OUT_BF16, TTB_ACT_GELU_NEW>(p, p.g[G_FC], mw + G_FC, map_a, lw.bfc, p.h, 4 * p.D, data, ctrl, rl, tmem_base);
+      gemm_phase<OUT_BF16, TTB_ACT_GELU_NEW>(p, p.g[G_FC], mw + G_FC, map_a, lw.bfc, p.h, 4 * p.D, data, ctrl, rl);
       AS_SYNC_UNLESS_LAST(5, l);
     }
     if (p.phase_mask & PH_PROJ2) {
-      gemm_phase<OUT_PARTIAL, TTB_ACT_NONE>(p, p.g[G_PROJ2], mw + G_PROJ2, map_h, nullptr, nullptr, 0, data, ctrl, rl, tmem_base);
+      gemm_phase<OUT_PARTIAL, TTB_ACT_NONE>(p, p.g[G_PROJ2], mw + G_PROJ2, map_h, nullptr, nullptr, 0, data, ctrl, rl);
       AS_SYNC_UNLESS_LAST(6, l);
     }
     if (p.phase_mask & PH_LN1) {
@@ -1036,14 +1022,7 @@ __global__ void __launch_bounds__(AS_THREADS, 1) ar_step_kernel(const __grid_con
     }
   }
   if (p.phase_mask & PH_HEAD) {
-    gemm_phase<OUT_F32, TTB_ACT_NONE>(p, p.g[G_HEAD], p.maps + 4 * p.L, map_hn, p.b_head, p.logits, p.V, data, ctrl, rl, tmem_base);
-  }
-  // ---- teardown
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<256>(tmem_base);
+    gemm_phase<OUT_F32, TTB_ACT_NONE>(p, p.g[G_HEAD], p.maps + 4 * p.L, map_hn, p.b_head, p.logits, p.V, data, ctrl, rl);
   }
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     // every CTA has read the epoch before its first arrival, and all arrivals of this launch precede this point
@@ -1051,8 +1030,8 @@ __global__ void __launch_bounds__(AS_THREADS, 1) ar_step_kernel(const __grid_con
   }
 }
 
-// The attention phase alone as an ordinary (non-cooperative) launch: no TMEM, no grid barrier. Used by the "mixed" decode
-// mode, where the GEMMs / LayerNorms of the step stay separate kernels (faster at >= 64 candidates, see ar_engine.py).
+// The attention phase alone as an ordinary (non-cooperative) launch: no grid barrier. Used by the "mixed" decode
+// mode, where the GEMMs / LayerNorms of the step stay separate kernels (see ar_engine.py).
 __global__ void __launch_bounds__(AS_THREADS, 1) ar_attn_only_kernel(const __grid_constant__ AsParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* data = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -1067,7 +1046,7 @@ __global__ void __launch_bounds__(AS_THREADS, 1) ar_attn_only_kernel(const __gri
   if (p.attn_impl < 1) pdl_wait();  // qkv belongs to the c_attn GEMM before this point (TTB_PDL=1); the tensor-core form
                                     // waits inside, after it has requested its first cache tiles
   AsRole rl;
-  rl.stage = 0; rl.phase = 0; rl.acc_par = 0; rl.prefix_par = 0; rl.bar_target = 0;
+  rl.stage = 0; rl.phase = 0; rl.prefix_par = 0; rl.bar_target = 0;
   rl.ring_par[0] = rl.ring_par[1] = rl.ring_par[2] = rl.ring_par[3] = 0;
   const int l = p.layer_begin;
   if (p.attn_impl >= 1) attn_phase_mma(p, l, data, ctrl, rl, true);
@@ -1094,7 +1073,7 @@ __global__ void __launch_bounds__(AS_COMPACT_WARPS * 32, 2) ar_attn_compact_kern
   }
   __syncthreads();
   AsRole rl;
-  rl.stage = 0; rl.phase = 0; rl.acc_par = 0; rl.prefix_par = 0; rl.bar_target = 0;
+  rl.stage = 0; rl.phase = 0; rl.prefix_par = 0; rl.bar_target = 0;
   rl.ring_par[0] = rl.ring_par[1] = rl.ring_par[2] = rl.ring_par[3] = 0;
   attn_phase_mma(p, p.layer_begin, data, ctrl, rl, true);
   pdl_launch_dependents();
@@ -1124,7 +1103,7 @@ static int as_num_sms() {
   int dev = 0, n = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-  return n > 0 ? n : 148;
+  return n > 0 ? n : 132;
 }
 
 static int env_int(const char* name, int dflt) {

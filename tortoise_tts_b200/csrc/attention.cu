@@ -1,7 +1,7 @@
 // Attention kernels, head_dim 64.
 //  * attn_simt_kernel: general softmax(q k^T * scale + relpos_bias [+ causal]) v, online-softmax (flash) form,
 //    one query per thread, K/V tiles staged in shared memory as fp32. Used for prompt prefill, latents, CLVP and
-//    diffusion attention (until the tcgen05 path in flash_attn.cu takes the large shapes).
+//    diffusion attention (the wgmma path in flash_attn.cu takes the large shapes).
 //  * ar_decode_attn_kernel: single-query attention of every (candidate, head) over [shared prefix | own KV]
 //    for the GPT-2 sampler; memory-bound on the KV stream (HBM roofline), appends the new K/V.
 #include "common.cuh"
@@ -358,7 +358,6 @@ extern "C" int ttb_attention(const TtbAttnArgs* ap, void* stream) {
     TTB_CHECK_LAUNCH("attn_warp_kernel");
     return 0;
   }
-  if (flash_attention2_supported(a)) return flash_attention2_launch(a, st);
   if (flash_attention_supported(a)) return flash_attention_launch(a, st);
   dim3 grid((a.T + ATT_Q - 1) / ATT_Q, a.H, a.nseq);
   attn_simt_kernel<<<grid, ATT_Q, 0, st>>>(a);

@@ -26,5 +26,5 @@ extern "C" int ttb_device_ok(void) {
   if (cudaGetDevice(&dev) != cudaSuccess) return 0;
   cudaDeviceProp p;
   if (cudaGetDeviceProperties(&p, dev) != cudaSuccess) return 0;
-  return p.major == 10 ? 1 : 0;
+  return (p.major == 9 && p.minor == 0) ? 1 : 0;
 }

@@ -1,5 +1,5 @@
-// Common device helpers for the tortoise-b200 kernels (sm_100a only).
-// PTX wrappers: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld), fences.
+// Common device helpers for the tortoise-b200 kernels (sm_90a only).
+// PTX wrappers: mbarrier, TMA (cp.async.bulk.tensor), wgmma (fence / mma_async / commit / wait), fences.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -25,13 +25,11 @@ int check_cuda(cudaError_t e, const char* what);
 // first access to global memory that an earlier kernel may have written (and before its own first global write).
 // Launched the ordinary way both instructions are no-ops. With TTB_PDL=1 the host launches these kernels with
 // cudaLaunchAttributeProgrammaticStreamSerialization: the next kernel's CTAs are scheduled, run their prologue
-// (barrier init, TMEM allocation, descriptor prefetch) and park in griddepcontrol.wait while the previous kernel
-// drains, which removes the kernel-to-kernel launch gap that dominates the ~10 us decode-step kernels.
-// Round 1 (profiles/bench_r01_pdl.txt): with the trigger at the very TOP of every kernel PDL was correct but slower
-// (AR 1346 -> 1445 ms): the dependent's CTAs became resident at once and took registers / shared memory away from the
-// kernel still running. Round 2 moved every trigger to the kernel's TAIL (GEMM: once all loads of the CTA are issued and
-// its accumulator is complete; LayerNorm: after its loads; others: at exit): AR 1246 -> 1187 ms with TTB_PDL=1
-// (gpurun_out/r2e, profiles/bench_r02_*.json). On by default; TTB_PDL=0 restores plain launches.
+// (barrier init, descriptor prefetch) and park in griddepcontrol.wait while the previous kernel drains, which removes
+// the kernel-to-kernel launch gap that dominates the short decode-step kernels. The triggers sit at the kernels' TAILS
+// (GEMM: once all loads of the CTA are issued and its accumulator is complete; LayerNorm: after its loads; others: at
+// exit): a trigger at the top makes the dependent's CTAs resident at once, and they take registers / shared memory
+// away from the kernel still running. On by default; TTB_PDL=0 restores plain launches.
 TTB_DEVINL void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 TTB_DEVINL void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
@@ -39,7 +37,7 @@ inline bool pdl_enabled() {
   static int v = -1;
   if (v < 0) {
     const char* e = getenv("TTB_PDL");
-    v = (e && e[0] == '0') ? 0 : 1;       // default on since round 2 (triggers at the kernel tails)
+    v = (e && e[0] == '0') ? 0 : 1;
   }
   return v == 1;
 }
@@ -154,7 +152,7 @@ TTB_DEVINL void mbar_arrive(uint64_t* bar) {
 // try_wait with a suspend-time hint: the waiting warp is parked by the hardware until the phase completes (or the hint
 // expires) instead of re-issuing the poll every few cycles -- the polls of the waiting roles (epilogue warps during a
 // mainloop, the single-lane TMA / MMA issuers) otherwise take issue slots from the warps doing the work on the same
-// scheduler (ncu, round 1: 40 % of the instructions executed by the flash-attention kernel were barrier polls).
+// scheduler.
 // TTB_MBAR_HINT_NS=0 at build time restores the plain poll loop (A/B).
 #ifndef TTB_MBAR_HINT_NS
 #define TTB_MBAR_HINT_NS 20000
@@ -206,100 +204,89 @@ TTB_DEVINL void tma_prefetch_l2_3d(const CUtensorMap* map, int c0, int c1, int c
                : "memory");
 }
 
-// ------------------------------------------------------------------ tcgen05
-TTB_DEVINL void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-TTB_DEVINL void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// ------------------------------------------------------------------ wgmma (Hopper warpgroup MMA)
+// A warpgroup = 4 consecutive warps whose first warp index is a multiple of 4. All 128 threads issue the instruction;
+// the fp32 accumulator lives in their registers: for m64nN, register i of lane l of warp w holds
+//   row = 16 w + l / 4 + 8 ((i >> 1) & 1),   column = 8 (i >> 2) + 2 (l & 3) + (i & 1).
+TTB_DEVINL void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+TTB_DEVINL void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+TTB_DEVINL void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+TTB_DEVINL void named_barrier(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
-template <int kCols>
-TTB_DEVINL void tmem_alloc(uint32_t* smem_dst) {  // one full warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int kCols>
-TTB_DEVINL void tmem_dealloc(uint32_t taddr) {  // same warp that allocated
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-
-// SM100 shared-memory matrix descriptor, K-major operand, SWIZZLE_128B, bf16:
-//   rows of 64 elements (128 B), 8-row swizzle atoms of 1024 B (SBO = 1024), LBO ignored (=1),
-//   descriptor version 1 (bits 46-47), layout type 2 = SWIZZLE_128B (bits 61-63).
-// (cute::UMMA::SmemDescriptor, cute/arch/mma_sm100_desc.hpp; canonical K-major layout in
-//  cute/atom/mma_traits_sm100.hpp make_umma_desc<Major::K>)
-TTB_DEVINL uint64_t umma_desc_kmajor_sw128(uint32_t smem_addr) {
+// Shared-memory matrix descriptor (sm_90), K-major operand, SWIZZLE_128B, bf16:
+//   rows of 64 elements (128 B), 8-row swizzle atoms of 1024 B (SBO = 1024), LBO ignored (=1), layout type 1 =
+//   128-byte swizzle (bits 62-63). (cute::GmmaDescriptor, cute/arch/mma_sm90_desc.hpp)
+TTB_DEVINL uint64_t wgmma_desc_kmajor_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);        // start address
   d |= (uint64_t)1 << 16;                             // leading byte offset (unused for swizzled K-major)
   d |= (uint64_t)(1024 >> 4) << 32;                   // stride byte offset: 8 rows * 128 B
-  d |= (uint64_t)1 << 46;                             // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;                             // SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                             // SWIZZLE_128B
   return d;
 }
-// MN-major operand (e.g. V [keys, 64 dims] used as B[N=64 dims, K=keys]), SWIZZLE_128B:
+// MN-major operand (e.g. V [keys, 64 dims] used as B[N=64 dims, K=keys], transposed by the instruction), SWIZZLE_128B:
 //   64 MN-elements contiguous (128 B) per K index; 8 K-rows per 1024-B atom (SBO = 1024);
 //   LBO = byte distance between 64-wide MN groups.
-TTB_DEVINL uint64_t umma_desc_mnmajor_sw128(uint32_t smem_addr, uint32_t lbo_bytes) {
+TTB_DEVINL uint64_t wgmma_desc_mnmajor_sw128(uint32_t smem_addr, uint32_t lbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
 
-// Instruction descriptor for kind::f16 with bf16 A/B, fp32 accumulate (cute::UMMA::InstrDescriptor).
-TTB_DEVINL constexpr uint32_t umma_idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4)                         // c_format = F32
-         | (1u << 7)                       // a_format = BF16
-         | (1u << 10)                      // b_format = BF16
-         | ((uint32_t)a_mn_major << 15)    // a_major
-         | ((uint32_t)b_mn_major << 16)    // b_major
-         | ((uint32_t)(N >> 3) << 17)      // n_dim
-         | ((uint32_t)(M >> 4) << 24);     // m_dim
+// D[registers] (+)= A[smem] * B[smem]^T (both K-major); scale_d == 0 overwrites D.
+TTB_DEVINL void wgmma_m64n16k16_bf16_ss(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(desc_a), "l"(desc_b), "r"(scale_d));
+}
+TTB_DEVINL void wgmma_m64n32k16_bf16_ss(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(desc_a), "l"(desc_b), "r"(scale_d));
+}
+TTB_DEVINL void wgmma_m64n64k16_bf16_ss(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(desc_a), "l"(desc_b), "r"(scale_d));
+}
+// A from registers (the m16n8k16 A-fragment layout per warp), B from smem; TNSPB = 1: B is MN-major.
+template <int TNSPB>
+TTB_DEVINL void wgmma_m64n64k16_bf16_rs(float* d, const uint32_t* a, uint64_t desc_b, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, %38;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d), "n"(TNSPB));
 }
 
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread.
-TTB_DEVINL void umma_bf16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+// The k-block of one consumer warpgroup: acc[64 x BN] (+)= A[64 rows x 64] * B[BN rows x 64]^T, both K-major SWIZZLE_128B
+// tiles in shared memory (sa = this warpgroup's 64 rows). BN = 32: one n32 instruction per k16, else BN / 64 n64 ones.
+template <int BN>
+TTB_DEVINL void gemm_mma_kblock(float* acc, uint32_t sa, uint32_t sb, bool first) {
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const uint64_t da = wgmma_desc_kmajor_sw128(sa + k * 32);
+    const uint32_t sc = (first && k == 0) ? 0u : 1u;
+    if constexpr (BN == 32) {
+      wgmma_m64n32k16_bf16_ss(acc, da, wgmma_desc_kmajor_sw128(sb + k * 32), sc);
+    } else {
+#pragma unroll
+      for (int nb = 0; nb < BN / 64; ++nb)
+        wgmma_m64n64k16_bf16_ss(acc + nb * 32, da, wgmma_desc_kmajor_sw128(sb + nb * 8192 + k * 32), sc);
+    }
+  }
+  wgmma_commit();
 }
-// mbarrier arrive when all previously issued tcgen05.mma of this thread have completed
-TTB_DEVINL void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// TMEM -> registers: 32 lanes x 32 consecutive 32-bit columns (thread i of the warp gets lane base+i)
-TTB_DEVINL void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-TTB_DEVINL void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// registers -> TMEM, same shape as tmem_ld_32x32b_x32
-TTB_DEVINL void tmem_st_32x32b_x32(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]),
-        "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]),
-        "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-TTB_DEVINL void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 }  // namespace ttb

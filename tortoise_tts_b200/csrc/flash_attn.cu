@@ -1,15 +1,16 @@
-// tcgen05 flash attention, head_dim 64, bf16 in/out, fp32 softmax statistics.
+// wgmma flash attention, head_dim 64, bf16 in/out, fp32 softmax statistics.
 //
 //   out = softmax(q k^T * scale + relpos_bias[h][kj - qi] (+ causal mask)) v      per (sequence, head)
 //
 // One CTA = 128 queries of one (sequence, head); KV streamed in tiles of 64 keys by TMA (2 stages) straight out of
 // the token-major qkv buffer (3-D tensor map, out-of-range rows zero-filled).
-//   warp 0      : TMA producer (Q once, then K/V tiles)
-//   warp 1      : TMEM allocator + MMA issuer:  S = Q K^T (UMMA 128x64x16, K-major A/B)  and
-//                 O_j = P V (A = P written to smem by the softmax warps, B = V tile used MN-major as loaded)
-//   warps 2..5  : softmax; thread r owns query row r (TMEM lane r): tcgen05.ld S row -> scale/bias/mask -> running
-//                 max/sum in registers -> P (bf16) to swizzled smem -> after the PV MMA, tcgen05.ld O_j and
-//                 accumulate o = o*corr + O_j in registers (no TMEM read-modify-write).
+//   warps 0..3, 4..7 : two consumer warpgroups of 64 queries each, sharing every K/V tile. Per tile:
+//                      S = Q K^T (wgmma m64n64k16, both operands K-major in shared memory) -> scale/bias/mask and the
+//                      running max/sum in registers (a query row lives in the 4 lanes of a quad) -> P (bf16) packed
+//                      into the A fragments of O += P V (wgmma with A from registers, B = V tile used MN-major as
+//                      loaded). O stays in registers.
+//   warp 8           : TMA producer (Q once, then K/V tiles)
+// The two warpgroups run independently, so while one does its softmax the tensor core serves the other.
 // Replaces the materialised [H, T, T] score tensors of QKVAttentionLegacy (arch_util.py:60-77), HF GPT2Attention._attn
 // and xtransformers Attention (xtransformers.py:660-712).
 #include <type_traits>
@@ -21,28 +22,23 @@ namespace ttb {
 
 constexpr int FA_BM = 128;   // queries per CTA
 constexpr int FA_BN = 64;    // keys per tile
-constexpr int FA_THREADS = 192;
+constexpr int FA_CONSUMERS = 256;
+constexpr int FA_PRODUCER_WARP = 8;
+constexpr int FA_THREADS = FA_CONSUMERS + 32;
 constexpr int FA_STAGES = 2;
 
 struct FaSmem {
   static constexpr int Q_BYTES = FA_BM * 64 * 2;          // 16 KB
   static constexpr int K_BYTES = FA_BN * 64 * 2;          // 8 KB
   static constexpr int V_BYTES = FA_BN * 64 * 2;          // 8 KB
-  static constexpr int P_BYTES = FA_BM * FA_BN * 2;       // 16 KB
   static constexpr int Q_OFF = 0;
   static constexpr int KV_OFF = Q_BYTES;
-  static constexpr int P_OFF = KV_OFF + FA_STAGES * (K_BYTES + V_BYTES);
-  static constexpr int BIAS_OFF = P_OFF + P_BYTES;        // 192 floats
+  static constexpr int BIAS_OFF = KV_OFF + FA_STAGES * (K_BYTES + V_BYTES);   // 192 floats
   static constexpr int BAR_OFF = BIAS_OFF + 192 * 4;
   static constexpr int TOTAL = BAR_OFF + 16 * 8 + 1024;
 };
 
-// DBUF (round-2 experiment, TTB_FA_DBUF=1, not yet run on hardware): S is double-buffered in TMEM and Q K_{j+1}^T is
-// issued BEFORE the MMA thread waits for P_j, so the softmax of tile j overlaps the score MMA of tile j+1 instead of
-// waiting behind [P V_j, Q K_{j+1}^T]. The softmax threads then wait for o_full(j-1) themselves before they touch O
-// (lazy rescale) or overwrite the single P buffer. With DBUF = false the kernel is unchanged.
-template <int MINB, bool DBUF = false>
-__global__ void __launch_bounds__(FA_THREADS, MINB)
+__global__ void __launch_bounds__(FA_THREADS, 2)
 flash_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                      const __grid_constant__ CUtensorMap map_v, TtbAttnArgs a) {
   extern __shared__ uint8_t smem_raw[];
@@ -51,11 +47,6 @@ flash_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
   uint64_t* q_full = bars + 0;
   uint64_t* kv_full = bars + 1;            // [FA_STAGES]
   uint64_t* kv_empty = bars + 1 + FA_STAGES;
-  constexpr int NS = DBUF ? 2 : 1;         // score buffers in TMEM
-  uint64_t* s_full = bars + 1 + 2 * FA_STAGES;   // [NS]
-  uint64_t* p_full = s_full + NS;
-  uint64_t* o_full = s_full + NS + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(s_full + NS + 2);
   float* sbias = reinterpret_cast<float*>(smem + FaSmem::BIAS_OFF);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -70,27 +61,18 @@ flash_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
   const int kvc2 = a.kv_headmajor ? h : seq;
   const int ntiles = (kv_end + FA_BN - 1) / FA_BN;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == FA_PRODUCER_WARP && lane == 0) {
     tma_prefetch_desc(&map_q);
     tma_prefetch_desc(&map_k);
     tma_prefetch_desc(&map_v);
     mbar_init(q_full, 1);
-    for (int s = 0; s < FA_STAGES; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], 1); }
-    for (int b = 0; b < NS; ++b) mbar_init(&s_full[b], 1);
-    mbar_init(p_full, 128);
-    mbar_init(o_full, 1);
+    for (int s = 0; s < FA_STAGES; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], 2); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<DBUF ? 256 : 128>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_wait();        // barrier init, TMEM allocation and descriptor prefetch above overlap the tail of the qkv GEMM
-  const uint32_t tmem_s = tmem_base;                        // columns [0, 64) (+ [64, 128) with DBUF)
-  const uint32_t tmem_o = tmem_base + (DBUF ? 128 : 64);    // 64 columns
+  pdl_wait();        // barrier init and descriptor prefetch above overlap the tail of the qkv GEMM
 
-  if (warp == 0) {
+  if (warp == FA_PRODUCER_WARP) {
     if (lane == 0) {
       mbar_arrive_expect_tx(q_full, FaSmem::Q_BYTES);
       tma_load_3d(smem + FaSmem::Q_OFF, &map_q, q_full, h * 64, q0, seq);
@@ -105,82 +87,23 @@ flash_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
         if (++stage == FA_STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = umma_idesc_bf16(FA_BM, FA_BN, 0, 0);   // S[128x64] = Q[128x64d] * K[64keys x 64d]^T
-      constexpr uint32_t idesc_o = umma_idesc_bf16(FA_BM, 64, 0, 1);      // O[128x64d] = P[128x64keys] * V (MN-major B)
-      const uint32_t sq = smem_u32(smem + FaSmem::Q_OFF);
-      const uint32_t sp = smem_u32(smem + FaSmem::P_OFF);
-      mbar_wait(q_full, 0);
-      int stage = 0; uint32_t phase = 0;
-      if constexpr (DBUF) {
-        // S_0 first; then per tile: S_{j+1} (other score buffer, next KV stage) BEFORE waiting for P_j, then P V_j
-        mbar_wait(&kv_full[0], 0);
-        tc_fence_after();
-        {
-          const uint32_t sk = smem_u32(smem + FaSmem::KV_OFF);
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            umma_bf16_ss(tmem_s, umma_desc_kmajor_sw128(sq + k * 32), umma_desc_kmajor_sw128(sk + k * 32), idesc_s, k != 0);
-          umma_commit(&s_full[0]);
-        }
-        for (int j = 0; j < ntiles; ++j) {
-          const int nstage = (stage + 1 == FA_STAGES) ? 0 : stage + 1;
-          const uint32_t nphase = (stage + 1 == FA_STAGES) ? (phase ^ 1) : phase;
-          if (j + 1 < ntiles) {
-            // score buffer (j+1)&1 was last read by the softmax of tile j-1, which arrived on p_full(j-1) afterwards
-            mbar_wait(&kv_full[nstage], nphase);
-            tc_fence_after();
-            const uint32_t sk = smem_u32(smem + FaSmem::KV_OFF + nstage * (FaSmem::K_BYTES + FaSmem::V_BYTES));
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-              umma_bf16_ss(tmem_s + (uint32_t)(((j + 1) & 1) * 64), umma_desc_kmajor_sw128(sq + k * 32),
-                           umma_desc_kmajor_sw128(sk + k * 32), idesc_s, k != 0);
-            umma_commit(&s_full[(j + 1) & 1]);
-          }
-          mbar_wait(p_full, j & 1);
-          tc_fence_after();
-          const uint32_t sv = smem_u32(smem + FaSmem::KV_OFF + stage * (FaSmem::K_BYTES + FaSmem::V_BYTES)) + FaSmem::K_BYTES;
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            umma_bf16_ss(tmem_o, umma_desc_kmajor_sw128(sp + k * 32), umma_desc_mnmajor_sw128(sv + k * 2048, 0), idesc_o, (j | k) != 0);
-          umma_commit(o_full);
-          umma_commit(&kv_empty[stage]);
-          stage = nstage; phase = nphase;
-        }
-      } else
-      for (int j = 0; j < ntiles; ++j) {
-        mbar_wait(&kv_full[stage], phase);
-        tc_fence_after();
-        const uint32_t sk = smem_u32(smem + FaSmem::KV_OFF + stage * (FaSmem::K_BYTES + FaSmem::V_BYTES));
-        const uint32_t sv = sk + FaSmem::K_BYTES;
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          umma_bf16_ss(tmem_s, umma_desc_kmajor_sw128(sq + k * 32), umma_desc_kmajor_sw128(sk + k * 32), idesc_s, k != 0);
-        umma_commit(s_full);
-        mbar_wait(p_full, j & 1);            // softmax consumed S_j and wrote P_j
-        tc_fence_after();
-#pragma unroll
-        for (int k = 0; k < 4; ++k)           // K (= keys) advances 16 rows of 128 B per step in the MN-major V tile
-          umma_bf16_ss(tmem_o, umma_desc_kmajor_sw128(sp + k * 32), umma_desc_mnmajor_sw128(sv + k * 2048, 0), idesc_o, (j | k) != 0);
-        umma_commit(o_full);
-        umma_commit(&kv_empty[stage]);
-        if (++stage == FA_STAGES) { stage = 0; phase ^= 1; }
-      }
-    }
+    __syncwarp();
   } else {
-    const int qd = warp & 3;
-    const int row = qd * 32 + lane;            // TMEM lane == query row inside the tile
-    const int st = threadIdx.x - 64;           // 0..127 among the softmax threads
-    const int qi = q0 + row;
+    const int wg = warp >> 2;
+    const int g = lane >> 2, t = lane & 3;
+    const int row0 = wg * 64 + (warp & 3) * 16 + g;   // this thread's query rows inside the tile: row0 and row0 + 8
     const float sl2 = a.scale * 1.4426950408889634f;
     const float* bias_h = a.bias ? a.bias + (long long)h * (2 * T - 1) + (T - 1) : nullptr;
-    // Running statistics in the log2 domain. O accumulates in TMEM across tiles (the PV MMA runs with
-    // enable-input-d); it is rescaled in place only when this row's max grows by more than 2^8 ("lazy rescale"),
-    // so P values stay <= 256 and the common case needs no TMEM round trip.
-    float m = -INFINITY, l = 0.f;
-    uint8_t* sp = smem + FaSmem::P_OFF;
-    const uint32_t lane_base = (uint32_t)(qd * 32) << 16;
+    // Running statistics in the log2 domain, per row half (hh = 0: row0, 1: row0 + 8); l is this thread's share of the
+    // row sum (reduced over the quad at the end). O is rescaled only when a row's max grows by more than 2^8 ("lazy
+    // rescale"), so P values stay <= 256.
+    float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+    float o[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] = 0.f;
+    const uint32_t sq = smem_u32(smem + FaSmem::Q_OFF) + wg * (64 * 128);
+    mbar_wait(q_full, 0);
+    int stage = 0; uint32_t phase = 0;
     for (int j = 0; j < ntiles; ++j) {
       const int k0 = j * FA_BN;
       // Tile classification (uniform over the CTA): far from the diagonal the T5 bias is saturated, i.e. constant
@@ -195,140 +118,107 @@ flash_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
       const bool fast = nomask && cbias_ok;
       if (bias_h && !fast) {
         // window of the Toeplitz bias table needed by this (q-tile, k-tile): rel = kj - qi in [k0-q0-127, k0-q0+63]
-        asm volatile("bar.sync 1, 128;" ::: "memory");   // previous tile's readers are done
-        for (int i = st; i < 191; i += 128) {
+        named_barrier(1, FA_CONSUMERS);                   // previous tile's readers are done
+        for (int i = threadIdx.x; i < 191; i += FA_CONSUMERS) {
           const int rel = k0 - q0 - 127 + i;
           sbias[i] = (rel > -T && rel < T) ? __ldg(bias_h + rel) * 1.4426950408889634f : 0.f;
         }
-        asm volatile("bar.sync 1, 128;" ::: "memory");
+        named_barrier(1, FA_CONSUMERS);
       }
-      // The rest of the tile is instantiated once per tile class: with one shared body the score registers of the two
-      // classes had to agree at the join, which cost the common (fast) class 64 register moves per tile (SASS of
-      // profiles/ncu_r02/fa_dbuf.ncu-rep: 42 IMAD.MOV + 22 MOV in a 100-instruction max block).
-      auto tile_body = [&](auto fast_tag) {
-      constexpr bool FAST = decltype(fast_tag)::value;
-      // S_j ready (without DBUF this also means that every earlier MMA, incl. P V of tile j-1, has retired)
-      mbar_wait(&s_full[DBUF ? (j & 1) : 0], DBUF ? ((j >> 1) & 1) : (j & 1));
-      tc_fence_after();
-      uint32_t r0[32], r1[32];
-      tmem_ld_32x32b_x32(tmem_s + (DBUF ? (uint32_t)((j & 1) * 64) : 0u) + lane_base, r0);
-      tmem_ld_32x32b_x32(tmem_s + (DBUF ? (uint32_t)((j & 1) * 64) : 0u) + lane_base + 32, r1);
-      tmem_ld_wait();
-      float mx = -INFINITY;
-      if constexpr (FAST) {
-        float mq[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};   // 4 independent chains (ILP)
+      mbar_wait(&kv_full[stage], phase);
+      const uint32_t sk = smem_u32(smem + FaSmem::KV_OFF + stage * (FaSmem::K_BYTES + FaSmem::V_BYTES));
+      const uint32_t sv = sk + FaSmem::K_BYTES;
+      // S[64 x 64 keys] = Q[64 x 64d] K[64 keys x 64d]^T
+      float s[32];
+      wgmma_fence();
 #pragma unroll
-        for (int c = 0; c < 32; ++c) mq[c & 3] = fmaxf(mq[c & 3], fmaxf(__uint_as_float(r0[c]), __uint_as_float(r1[c])));
-        mx = fmaxf(fmaxf(mq[0], mq[1]), fmaxf(mq[2], mq[3]));
-        mx = fmaf(mx, sl2, cb);
+      for (int k = 0; k < 4; ++k)
+        wgmma_m64n64k16_bf16_ss(s, wgmma_desc_kmajor_sw128(sq + k * 32), wgmma_desc_kmajor_sw128(sk + k * 32), k != 0);
+      wgmma_commit();
+      wgmma_wait<0>();
+      // register i: row half (i >> 1) & 1, key column c = 8 (i >> 2) + 2 t + (i & 1)
+      float mx[2] = {-INFINITY, -INFINITY};
+      if (fast) {
+#pragma unroll
+        for (int i = 0; i < 32; ++i) mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], s[i]);
+        mx[0] = fmaf(mx[0], sl2, cb);
+        mx[1] = fmaf(mx[1], sl2, cb);
       } else {
-        const int klim = min(T - k0, a.causal ? (qi - k0 + 1) : FA_BN);   // keys c < klim are visible to this row
 #pragma unroll
-        for (int c = 0; c < 64; ++c) {
-          float v = __uint_as_float(c < 32 ? r0[c] : r1[c - 32]) * sl2;
+        for (int i = 0; i < 32; ++i) {
+          const int hh = (i >> 1) & 1;
+          const int row = row0 + 8 * hh;
+          const int c = 8 * (i >> 2) + 2 * t + (i & 1);
+          const int klim = min(T - k0, a.causal ? (q0 + row - k0 + 1) : FA_BN);   // keys c < klim are visible to this row
+          float v = s[i] * sl2;
           if (bias_h) v += sbias[c - row + 127];
           v = (c < klim) ? v : -INFINITY;
-          if (c < 32) r0[c] = __float_as_uint(v); else r1[c - 32] = __float_as_uint(v);
-          mx = fmaxf(mx, v);
+          s[i] = v;
+          mx[hh] = fmaxf(mx[hh], v);
         }
       }
-      if constexpr (DBUF) {
-        // O (lazy rescale below) and the P buffer belong to P V_{j-1} until it has retired
-        if (j > 0) { mbar_wait(o_full, (j - 1) & 1); tc_fence_after(); }
+      float corr[2], cm[2];
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
+        mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
+        const bool grow = mx[hh] > m[hh] + 8.0f;         // also true for the first finite max (m = -inf)
+        const float m_new = grow ? mx[hh] : m[hh];
+        corr[hh] = grow ? exp2f(m[hh] - m_new) : 1.0f;   // exp2(-inf) = 0 on the first tile
+        m[hh] = m_new;
+        const float m_use = (m_new == -INFINITY) ? 0.f : m_new;
+        cm[hh] = fast ? cb - m_use : -m_use;
       }
-      const bool grow = mx > m + 8.0f;                 // also true for the first finite max (m = -inf)
-      const float m_new = grow ? mx : m;
-      const float corr = grow ? exp2f(m - m_new) : 1.0f;   // exp2(-inf) = 0 on the first tile
-      if (j > 0 && __any_sync(0xffffffffu, grow)) {
-        uint32_t t0[32];
-        tmem_ld_32x32b_x32(tmem_o + lane_base, t0);
-        tmem_ld_wait();
+      float psum[2] = {0.f, 0.f};
+      uint32_t pa[16];                                    // P as the A fragments of the four k16 steps of P V
 #pragma unroll
-        for (int d = 0; d < 32; ++d) t0[d] = __float_as_uint(__uint_as_float(t0[d]) * corr);
-        tmem_st_32x32b_x32(tmem_o + lane_base, t0);
-        tmem_ld_32x32b_x32(tmem_o + lane_base + 32, t0);
-        tmem_ld_wait();
-#pragma unroll
-        for (int d = 0; d < 32; ++d) t0[d] = __float_as_uint(__uint_as_float(t0[d]) * corr);
-        tmem_st_32x32b_x32(tmem_o + lane_base + 32, t0);
-        tmem_st_wait();
+      for (int i = 0; i < 32; i += 2) {
+        const int hh = (i >> 1) & 1;
+        const float p0 = fast ? exp2f(fmaf(s[i], sl2, cm[hh])) : exp2f(s[i] + cm[hh]);
+        const float p1 = fast ? exp2f(fmaf(s[i + 1], sl2, cm[hh])) : exp2f(s[i + 1] + cm[hh]);
+        psum[hh] += p0 + p1;
+        pa[i >> 1] = pack_bf16(p0, p1);
       }
-      const float m_use = (m_new == -INFINITY) ? 0.f : m_new;
-      float psum = 0.f;
-      uint32_t pk[32];
-      if constexpr (FAST) {
-        const float cm = cb - m_use;
-        float ps[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
-        for (int c = 0; c < 64; c += 2) {
-          const float p0 = exp2f(fmaf(__uint_as_float(c < 32 ? r0[c] : r1[c - 32]), sl2, cm));
-          const float p1 = exp2f(fmaf(__uint_as_float(c < 32 ? r0[c + 1] : r1[c - 31]), sl2, cm));
-          ps[(c >> 1) & 3] += p0 + p1;
-          pk[c >> 1] = pack_bf16(p0, p1);
-        }
-        psum = (ps[0] + ps[1]) + (ps[2] + ps[3]);
+      for (int hh = 0; hh < 2; ++hh) l[hh] = l[hh] * corr[hh] + psum[hh];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) o[i] *= corr[(i >> 1) & 1];
+      // O[64 x 64d] += P[64 x 64 keys] V[64 keys x 64d]; the key index advances 16 rows of 128 B per step in the V tile
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma_m64n64k16_bf16_rs<1>(o, pa + 4 * k, wgmma_desc_mnmajor_sw128(sv + k * 2048, 0), 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      if ((threadIdx.x & 127) == 0) mbar_arrive(&kv_empty[stage]);
+      if (++stage == FA_STAGES) { stage = 0; phase ^= 1; }
+    }
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 1);
+      l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 2);
+      const int qi = q0 + row0 + 8 * hh;
+      if (qi >= Tq) continue;
+      const float inv = 1.0f / l[hh];
+      if (a.lse) {
+        // partial-attention mode: normalised O in fp32 + log2-sum-exp, to be merged with another key range
+        float* op = a.out_f32 + ((long long)seq * Tq + qi) * a.ldo + h * 64 + 2 * t;
+#pragma unroll
+        for (int nb = 0; nb < 8; ++nb)
+          *reinterpret_cast<float2*>(op + 8 * nb) = make_float2(o[4 * nb + 2 * hh] * inv, o[4 * nb + 2 * hh + 1] * inv);
+        if (t == 0) a.lse[((long long)seq * Tq + qi) * a.H + h] = m[hh] + log2f(l[hh]);
       } else {
+        __nv_bfloat16* op = reinterpret_cast<__nv_bfloat16*>(a.out) + ((long long)seq * Tq + qi) * a.ldo + h * 64 + 2 * t;
 #pragma unroll
-        for (int c = 0; c < 64; c += 2) {
-          const float p0 = exp2f(__uint_as_float(c < 32 ? r0[c] : r1[c - 32]) - m_use);
-          const float p1 = exp2f(__uint_as_float(c < 32 ? r0[c + 1] : r1[c - 31]) - m_use);
-          psum += p0 + p1;
-          pk[c >> 1] = pack_bf16(p0, p1);
-        }
+        for (int nb = 0; nb < 8; ++nb)
+          *reinterpret_cast<uint32_t*>(op + 8 * nb) = pack_bf16(o[4 * nb + 2 * hh] * inv, o[4 * nb + 2 * hh + 1] * inv);
       }
-      l = l * corr + psum;
-      m = m_new;
-      // P row (64 bf16 = 128 B) into the K-major SWIZZLE_128B layout: 16-byte chunk c8 lands at (c8 ^ (row & 7))
-      uint4* prow = reinterpret_cast<uint4*>(sp + row * 128);
-#pragma unroll
-      for (int c8 = 0; c8 < 8; ++c8)
-        prow[c8 ^ (row & 7)] = make_uint4(pk[4 * c8], pk[4 * c8 + 1], pk[4 * c8 + 2], pk[4 * c8 + 3]);
-      fence_proxy_async();
-      tc_fence_before();
-      mbar_arrive(p_full);
-      };
-      if (fast) tile_body(std::true_type{}); else tile_body(std::false_type{});
-    }
-    // all P V products have been issued; wait for the last one and read the accumulated O row
-    mbar_wait(o_full, (ntiles - 1) & 1);
-    tc_fence_after();
-    float o[64];
-    {
-      uint32_t t0[32], t1[32];
-      tmem_ld_32x32b_x32(tmem_o + lane_base, t0);
-      tmem_ld_32x32b_x32(tmem_o + lane_base + 32, t1);
-      tmem_ld_wait();
-#pragma unroll
-      for (int d = 0; d < 32; ++d) { o[d] = __uint_as_float(t0[d]); o[d + 32] = __uint_as_float(t1[d]); }
-    }
-    tc_fence_before();
-    if (qi < Tq && a.lse) {
-      // partial-attention mode: normalised O in fp32 + log2-sum-exp, to be merged with another key range
-      const float inv = 1.0f / l;
-      float* op = a.out_f32 + ((long long)seq * Tq + qi) * a.ldo + h * 64;
-#pragma unroll
-      for (int i = 0; i < 16; ++i)
-        reinterpret_cast<float4*>(op)[i] = make_float4(o[4 * i] * inv, o[4 * i + 1] * inv, o[4 * i + 2] * inv, o[4 * i + 3] * inv);
-      a.lse[((long long)seq * Tq + qi) * a.H + h] = m + log2f(l);
-    } else if (qi < Tq) {
-      const float inv = 1.0f / l;
-      __nv_bfloat16* op = reinterpret_cast<__nv_bfloat16*>(a.out) + ((long long)seq * Tq + qi) * a.ldo + h * 64;
-      uint4* o4 = reinterpret_cast<uint4*>(op);
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-        o4[i] = make_uint4(pack_bf16(o[8 * i] * inv, o[8 * i + 1] * inv), pack_bf16(o[8 * i + 2] * inv, o[8 * i + 3] * inv),
-                           pack_bf16(o[8 * i + 4] * inv, o[8 * i + 5] * inv), pack_bf16(o[8 * i + 6] * inv, o[8 * i + 7] * inv));
     }
   }
   pdl_launch_dependents();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<DBUF ? 256 : 128>(tmem_base);
-  }
 }
 
-static int g_fa_mode = -1;  // 1 = tcgen05 (default), 0 = SIMT (TTB_ATTN_IMPL=simt)
+static int g_fa_mode = -1;  // 1 = wgmma (default), 0 = SIMT (TTB_ATTN_IMPL=simt)
 
 bool flash_attention_supported(const TtbAttnArgs& a) {
   if (g_fa_mode < 0) {
@@ -336,7 +226,7 @@ bool flash_attention_supported(const TtbAttnArgs& a) {
     g_fa_mode = (e && strcmp(e, "simt") == 0) ? 0 : 1;
   }
   if (!g_fa_mode) return false;
-  if (a.kv || a.lse) return true;      // split Q / KV tensors and LSE output exist only in the tcgen05 kernel
+  if (a.kv || a.lse) return true;      // split Q / KV tensors and LSE output exist only in the wgmma kernel
   return a.T >= 64 && (a.ld % 8) == 0;
 }
 
@@ -355,33 +245,14 @@ int flash_attention_launch(const TtbAttnArgs& a, cudaStream_t st) {
     mv = mk;
   }
   if (a.lse && !a.out_f32) { set_error("flash attention: lse output needs out_f32"); return -1; }
-  static int dbuf = -1;
-  if (dbuf < 0) { const char* e = getenv("TTB_FA_DBUF"); dbuf = (e && e[0] == '0') ? 0 : 1; }   // default on (0.109 -> 0.098 ms)
-  if (dbuf) {
-    static bool attr = false;
-    if (!attr) {
-      cudaError_t r = cudaFuncSetAttribute(flash_attn_tc_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, FaSmem::TOTAL);
-      if (r != cudaSuccess) return check_cuda(r, "cudaFuncSetAttribute(flash_attn dbuf)");
-      attr = true;
-    }
-    dim3 grid_d((a.T + FA_BM - 1) / FA_BM, a.H, a.nseq);
-    const cudaError_t led = launch_pdl(flash_attn_tc_kernel<2, true>, grid_d, dim3(FA_THREADS), (size_t)FaSmem::TOTAL, st, mq, mk, mv, a);
-    if (led != cudaSuccess) return check_cuda(led, "flash_attn_tc_kernel<dbuf> launch");
-    TTB_CHECK_LAUNCH("flash_attn_tc_kernel<dbuf>");
-    return 0;
-  }
-  static int occ = 0;
-  if (!occ) {
-    const char* e = getenv("TTB_FA_OCC");       // CTAs per SM the kernel is compiled for (register cap): 2 (default) or 3
-    occ = (e && atoi(e) == 3) ? 3 : 2;
-    cudaError_t r = (occ == 3)
-        ? cudaFuncSetAttribute(flash_attn_tc_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, FaSmem::TOTAL)
-        : cudaFuncSetAttribute(flash_attn_tc_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, FaSmem::TOTAL);
-    if (r != cudaSuccess) { occ = 0; return check_cuda(r, "cudaFuncSetAttribute(flash_attn)"); }
+  static bool attr = false;
+  if (!attr) {
+    cudaError_t r = cudaFuncSetAttribute(flash_attn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FaSmem::TOTAL);
+    if (r != cudaSuccess) return check_cuda(r, "cudaFuncSetAttribute(flash_attn)");
+    attr = true;
   }
   dim3 grid((a.T + FA_BM - 1) / FA_BM, a.H, a.nseq);
-  const cudaError_t le = (occ == 3) ? launch_pdl(flash_attn_tc_kernel<3>, grid, dim3(FA_THREADS), (size_t)FaSmem::TOTAL, st, mq, mk, mv, a)
-                                    : launch_pdl(flash_attn_tc_kernel<2>, grid, dim3(FA_THREADS), (size_t)FaSmem::TOTAL, st, mq, mk, mv, a);
+  const cudaError_t le = launch_pdl(flash_attn_tc_kernel, grid, dim3(FA_THREADS), (size_t)FaSmem::TOTAL, st, mq, mk, mv, a);
   if (le != cudaSuccess) return check_cuda(le, "flash_attn_tc_kernel launch");
   TTB_CHECK_LAUNCH("flash_attn_tc_kernel");
   return 0;

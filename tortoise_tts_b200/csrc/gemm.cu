@@ -1,13 +1,14 @@
-// tcgen05 GEMM / conv-as-GEMM for sm_100a.
+// wgmma GEMM / conv-as-GEMM for sm_90a.
 //
 //   D[b, m, n] = epilogue( sum_{tap, k} A[b, m + tap*1 - pad, k] * W[n, tap*K + k] )
 //
 // A: bf16 activations, token-major [batch, rows, K] (K contiguous), streamed by TMA (3-D map; out-of-range
 //    rows are zero-filled by the TMA unit, which is exactly Conv1d zero padding).
 // W: bf16 weights [N, taps*K] (K-major), streamed by TMA.
-// Accumulator: fp32 in TMEM (128 lanes x BN columns), written by tcgen05.mma (UMMA 128xBNx16, cta_group::1).
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM alloc + MMA issuer, warps 2..5 = epilogue
-// (tcgen05.ld 32x32b -> bias / activation / residual -> global).
+// Accumulator: fp32 in the registers of two consumer warpgroups (64 rows x BN columns each), written by
+// wgmma.mma_async (m64nNk16, both operands from shared memory).
+// Warp roles (288 threads): warps 0..7 = the two consumer warpgroups (main loop, then the epilogue: accumulator staged
+// through shared memory -> bias / activation / residual -> global), warp 8 = TMA producer.
 //
 // Replaces, behind the C-ABI, every dense contraction of the reference hot path that PyTorch dispatches to
 // cuBLAS / cuDNN: HF Conv1D addmm (GPT-2 c_attn/c_proj/c_fc, via autoregressive.py:150-163), nn.Linear
@@ -107,7 +108,9 @@ int make_tensor_map_bf16_nd(CUtensorMap* out, const void* ptr, int rank, const u
 // ------------------------------------------------------------------ kernel
 constexpr int BM = 128;
 constexpr int BK = 64;
-constexpr int GEMM_THREADS = 192;
+constexpr int GEMM_CONSUMERS = 256;      // two warpgroups: wgmma + epilogue
+constexpr int PRODUCER_WARP = 8;          // TMA producer
+constexpr int GEMM_THREADS = GEMM_CONSUMERS + 32;
 
 struct GemmEpilogue {
   const float* bias;       // [N] or null
@@ -135,13 +138,36 @@ struct GemmSmem {
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int BAR_OFF = STAGES * STAGE_BYTES;
   static constexpr int TOTAL = BAR_OFF + (2 * STAGES + 1) * 8 + 16 + 1024;  // + alignment slack
+  // once the main loop has retired, the pipeline stages hold the staged fp32 accumulator tile [128][BN + 8]
+  static_assert(BM * (BN + 8) * 4 <= BAR_OFF, "accumulator tile must fit the idle pipeline stages");
+  static_assert(TOTAL <= 227 * 1024, "GEMM shared memory");
 };
 
-// SPLIT_PRODUCER (experiment, variant 5): the A tiles are issued by warp 0 and the B tiles by lane 0 of the first epilogue
-// warp (idle during the mainloop). Measured in round 1: one CTA receives its operands at ~46 B/clk whatever the stage
-// count or tile width, two co-resident CTAs at twice that; if the limit is per issuing thread, two issuers double it.
+// Main loop of the two consumer warpgroups over num_kb pipeline stages, starting at (stage, phase). One thread per
+// warpgroup releases a stage once the wgmma group that read it has retired (one group stays in flight). RELEASE(bar)
+// performs the arrive (plain, or on every CTA of a cluster).
+template <int BN, int STAGES, typename Release>
+TTB_DEVINL void gemm_consumer_mainloop(float* acc, uint8_t* smem, int stage_bytes, int a_bytes, uint64_t* full_bar,
+                                       uint64_t* empty_bar, int num_kb, int& stage, uint32_t& phase, int wg, bool leader,
+                                       Release release) {
+  int prev = -1;
+  for (int kb = 0; kb < num_kb; ++kb) {
+    mbar_wait(&full_bar[stage], phase);
+    const uint32_t sa = smem_u32(smem + stage * stage_bytes);
+    gemm_mma_kblock<BN>(acc, sa + wg * (64 * BK * 2), sa + a_bytes, kb == 0);
+    wgmma_wait<1>();
+    if (prev >= 0 && leader) release(&empty_bar[prev]);
+    prev = stage;
+    if (++stage == STAGES) { stage = 0; phase ^= 1; }
+  }
+  wgmma_wait<0>();
+  if (prev >= 0 && leader) release(&empty_bar[prev]);
+}
+
+// SPLIT_PRODUCER (experiment, variant 5): the A tiles are issued by lane 0 and the B tiles by lane 1 of the producer warp:
+// if the rate at which one CTA receives its operands is limited per issuing thread, two issuers double it.
 template <int BN, int STAGES, bool SPLIT_PRODUCER = false>
-__global__ void __launch_bounds__(GEMM_THREADS, BN <= 128 ? 2 : 1)
+__global__ void __launch_bounds__(GEMM_THREADS, BN <= 64 ? 2 : 1)
 gemm_bf16_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, int M, int N,
                     int K, int taps, int pad, int a_batch_mul, int kb_per_split, GemmEpilogue ep,
                     unsigned long long* trace) {
@@ -153,8 +179,6 @@ gemm_bf16_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_cons
   if (tr && threadIdx.x == 0) { tr[0] = global_timer_ns(); tr[1] = sm_id(); }
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* accum_bar = empty_bar + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_bar + 1);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -167,26 +191,21 @@ gemm_bf16_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_cons
   const int kb_begin = kb_per_split > 0 ? bz * kb_per_split : 0;
   const int num_kb = kb_per_split > 0 ? min(kb_per_split, kb_total - kb_begin) : kb_total;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == PRODUCER_WARP && lane == 0) {
     tma_prefetch_desc(&map_a);
     tma_prefetch_desc(&map_b);
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], SPLIT_PRODUCER ? 2 : 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(accum_bar, 1);
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], SPLIT_PRODUCER ? 2 : 1); mbar_init(&empty_bar[s], 2); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<BN>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   // W is a parameter (TtbGemmArgs.w_static): under programmatic dependent launch its tiles do not have to wait for the
   // kernels before this one. The first STAGES weight tiles go into the pipeline and the rest of this CTA's weight slab
   // is pulled into L2 BEFORE griddepcontrol.wait; only the activation tiles are requested after it. For the skinny
-  // decode GEMMs (a 64 KB slab per CTA, ~1.5 us of DRAM latency in front of a 4 us main loop) the weights then stream
-  // while the previous kernel (LayerNorm, which triggers its dependents early) is still running.
+  // decode GEMMs (a 64 KB slab per CTA in front of a short main loop) the weights then stream while the previous kernel
+  // (LayerNorm, which triggers its dependents early) is still running.
   int pre = 0;
   if constexpr (!SPLIT_PRODUCER) {
-    if (ep.wpre && warp == 0 && lane == 0) {
+    if (ep.wpre && warp == PRODUCER_WARP && lane == 0) {
       pre = num_kb < STAGES ? num_kb : STAGES;
       for (int kbi = 0; kbi < num_kb; ++kbi) {
         const int kb = kb_begin + kbi;
@@ -207,9 +226,9 @@ gemm_bf16_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_cons
   pdl_wait();                    // activations, residual and outputs belong to earlier kernels until here
   if (tr && threadIdx.x == 0) tr[2] = global_timer_ns();
 
-  if (warp == 0) {
+  if (warp == PRODUCER_WARP) {
     // ===== TMA producer =====
-    if (lane == 0) {
+    if (lane == 0 || (SPLIT_PRODUCER && lane == 1)) {
       int stage = 0; uint32_t phase = 0;
       for (int kbi = 0; kbi < pre; ++kbi) {                 // activation halves of the stages started above
         const int kb = kb_begin + kbi;
@@ -226,8 +245,13 @@ gemm_bf16_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_cons
         uint8_t* sa = smem + stage * L::STAGE_BYTES;
         uint8_t* sb = sa + L::A_BYTES;
         if constexpr (SPLIT_PRODUCER) {
-          mbar_arrive_expect_tx(&full_bar[stage], L::A_BYTES);
-          tma_load_3d(sa, &map_a, &full_bar[stage], kk, m0 + tap * ep.tap_dil - pad, bz * a_batch_mul);
+          if (lane == 0) {
+            mbar_arrive_expect_tx(&full_bar[stage], L::A_BYTES);
+            tma_load_3d(sa, &map_a, &full_bar[stage], kk, m0 + tap * ep.tap_dil - pad, bz * a_batch_mul);
+          } else {
+            mbar_arrive_expect_tx(&full_bar[stage], L::B_BYTES);
+            tma_load_3d(sb, &map_b, &full_bar[stage], tap * K + kk, n0, 0);
+          }
         } else {
           mbar_arrive_expect_tx(&full_bar[stage], L::STAGE_BYTES);
           tma_load_3d(sa, &map_a, &full_bar[stage], kk, m0 + tap * ep.tap_dil - pad, bz * a_batch_mul);
@@ -236,76 +260,40 @@ gemm_bf16_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_cons
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
-    pdl_launch_dependents();      // PDL trigger at the TAIL (round 1 had it at the top and lost 7 %): the dependents'
-                                  // CTAs may be scheduled once every CTA of this grid has all its loads in flight
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_bf16(BM, BN, 0, 0);
-      int stage = 0; uint32_t phase = 0;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        if (tr && kb == 0) tr[3] = global_timer_ns();
-        const uint32_t sa = smem_u32(smem + stage * L::STAGE_BYTES);
-        const uint32_t sb = sa + L::A_BYTES;
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k) {
-          const uint64_t da = umma_desc_kmajor_sw128(sa + k * 32);
-          const uint64_t db = umma_desc_kmajor_sw128(sb + k * 32);
-          umma_bf16_ss(tmem_base, da, db, idesc, (kb | k) != 0 ? 1u : 0u);
-        }
-        umma_commit(&empty_bar[stage]);  // frees the smem slot when these MMAs retire
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      umma_commit(accum_bar);
-      if (tr) tr[4] = global_timer_ns();
-    }
-    pdl_launch_dependents();
+    __syncwarp();
+    pdl_launch_dependents();      // PDL trigger at the TAIL: the dependents' CTAs may be scheduled once every CTA of this
+                                  // grid has all its loads in flight
   } else {
-    // ===== epilogue: warps 2..5; warp w may only touch TMEM lanes [32*(w%4), 32*(w%4)+32) =====
-    const int q = warp & 3;
-    if constexpr (SPLIT_PRODUCER) {
-      if (warp == 2 && lane == 0) {                 // second TMA issuer: the weight tiles
-        int stage = 0; uint32_t phase = 0;
-        for (int kbi = 0; kbi < num_kb; ++kbi) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          const int kb = kb_begin + kbi;
-          const int tap = kb / kblocks_per_tap;
-          const int kk = (kb - tap * kblocks_per_tap) * BK;
-          uint8_t* sb = smem + stage * L::STAGE_BYTES + L::A_BYTES;
-          mbar_arrive_expect_tx(&full_bar[stage], L::B_BYTES);
-          tma_load_3d(sb, &map_b, &full_bar[stage], tap * K + kk, n0, 0);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-      __syncwarp();
-    }
+    // ===== consumers: warpgroup wg owns accumulator rows [64 wg, 64 wg + 64); then the epilogue =====
+    const int wg = warp >> 2;
+    const int rb = warp >> 1;                         // 32-row block this warp finishes in the epilogue
     if (ep.residual) {
-      // these warps idle during the mainloop: pull the tile's residual rows into L2 meanwhile
-      const int m = m0 + q * 32 + lane;
-      if (m < M) {
+      // pull the tile's residual rows into L2 ahead of the epilogue
+      const int m = m0 + rb * 32 + lane;
+      if (m < M && !(warp & 1)) {
         const float* p = ep.residual + (long long)bz * ep.res_bstride + (long long)m * ep.ldr + n0;
 #pragma unroll
         for (int c = 0; c < BN; c += 32)
           if (n0 + c < N) asm volatile("prefetch.global.L2 [%0];" ::"l"(p + c));
       }
     }
-    mbar_wait(accum_bar, 0);
+    float acc[BN / 2];
+    int stage = 0; uint32_t phase = 0;
+    if (tr && threadIdx.x == 0) tr[3] = global_timer_ns();
+    gemm_consumer_mainloop<BN, STAGES>(acc, smem, L::STAGE_BYTES, L::A_BYTES, full_bar, empty_bar, num_kb, stage, phase, wg,
+                                       (threadIdx.x & 127) == 0, [](uint64_t* b) { mbar_arrive(b); });
+    if (tr && threadIdx.x == 0) tr[4] = global_timer_ns();
     pdl_launch_dependents();
-    tc_fence_after();
-    if (tr && threadIdx.x == 64) tr[5] = global_timer_ns();
-    // all MMAs have retired: the pipeline stages are idle and serve as the per-warp transpose scratch
-    gemm_epilogue_dispatch<BN>(tmem_base + ((uint32_t)(q * 32) << 16), n0, N, m0 + q * 32, M, lane, (long long)bz, ep,
-                               smem_u32(smem + (warp - 2) * EPI_SCRATCH_BYTES), nullptr);
-    tc_fence_before();
-    if (tr && threadIdx.x == 64) tr[6] = global_timer_ns();
+    // every wgmma of both warpgroups has retired: the pipeline stages are idle and take the staged accumulator tile
+    named_barrier(1, GEMM_CONSUMERS);
+    gemm_stage_accumulator<BN>(acc, smem_u32(smem), warp, lane);
+    named_barrier(1, GEMM_CONSUMERS);
+    if (tr && threadIdx.x == 0) tr[5] = global_timer_ns();
+    gemm_epilogue_dispatch<BN>(smem_u32(smem) + (uint32_t)(rb * 32 * (BN + 8)) * 4, n0, N, m0 + rb * 32, M, lane, (long long)bz,
+                               ep, warp & 1, 2);
+    if (tr && threadIdx.x == 0) tr[6] = global_timer_ns();
   }
   __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<BN>(tmem_base);
-  }
   if (tr && threadIdx.x == 0) tr[7] = global_timer_ns();
 }
 
@@ -347,7 +335,7 @@ __global__ void gemm_ref_kernel(const __nv_bfloat16* A, long long a_bstride, int
   if (ep.out_bf16) ep.out_bf16[(long long)bz * ep.outb_bstride + (long long)m * ep.ldob + on] = __float2bfloat16(v);
 }
 
-static int g_gemm_impl = -1;  // 0 = tcgen05, 1 = SIMT reference (bring-up only; TTB_GEMM_IMPL=ref)
+static int g_gemm_impl = -1;  // 0 = wgmma, 1 = SIMT reference (bring-up only; TTB_GEMM_IMPL=ref)
 static unsigned long long* g_gemm_trace = nullptr;   // ttb_debug_gemm_trace
 
 template <int BN, int STAGES, bool SPLIT_PRODUCER = false>
@@ -385,7 +373,6 @@ static int launch_tc(const TtbGemmArgs& g, const GemmEpilogue& ep, cudaStream_t 
 
 #include "gemm_persist.cuh"
 #include "gemm_mc.cuh"
-#include "gemm_2cta.cuh"
 
 namespace ttb {
 
@@ -395,12 +382,12 @@ static int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }
 
-template <int BN, int PSTAGES, int EW>
+template <int BN, int PSTAGES>
 static int launch_persistent(const TtbGemmArgs& g, const GemmEpilogue& ep, cudaStream_t st) {
   CUtensorMap ma, mb;
   const bool bcast = (g.batch == 1) || (g.a_bstride == 0);
@@ -409,10 +396,10 @@ static int launch_persistent(const TtbGemmArgs& g, const GemmEpilogue& ep, cudaS
   if (get_tensor_map_bf16(&ma, g.A, (uint64_t)g.K, (uint64_t)g.rows, a_d2, (uint64_t)g.lda, a_s2, BK, BM)) return -1;
   if (get_tensor_map_bf16(&mb, g.W, (uint64_t)g.K * g.taps, (uint64_t)g.N, 1, (uint64_t)g.K * g.taps,
                           (uint64_t)g.K * g.taps * g.N, BK, BN)) return -1;
-  using L = GemmPSmem<BN, PSTAGES, EW>;
+  using L = GemmPSmem<BN, PSTAGES>;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_tc_persistent_kernel<BN, PSTAGES, EW>,
+    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_tc_persistent_kernel<BN, PSTAGES>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL);
     if (e != cudaSuccess) return check_cuda(e, "cudaFuncSetAttribute(gemm persistent)");
     attr_set = true;
@@ -426,7 +413,7 @@ static int launch_persistent(const TtbGemmArgs& g, const GemmEpilogue& ep, cudaS
   const int m_tiles = (g.M + BM - 1) / BM, n_tiles = (g.N + BN - 1) / BN;
   const long long total = (long long)m_tiles * n_tiles * zdim;
   const int grid = (int)(total < num_sms() ? total : num_sms());
-  const cudaError_t le = launch_pdl(gemm_bf16_tc_persistent_kernel<BN, PSTAGES, EW>, dim3(grid), dim3(64 + 32 * EW), (size_t)L::TOTAL, st,
+  const cudaError_t le = launch_pdl(gemm_bf16_tc_persistent_kernel<BN, PSTAGES>, dim3(grid), dim3(GEMM_THREADS), (size_t)L::TOTAL, st,
       ma, mb, g.M, g.N, g.K, g.taps, g.pad, (bcast || g.splitk > 1) ? 0 : 1, kb_per_split, m_tiles, n_tiles, zdim, ep);
   if (le != cudaSuccess) return check_cuda(le, "gemm_bf16_tc_persistent_kernel launch");
   TTB_CHECK_LAUNCH("gemm_bf16_tc_persistent_kernel");
@@ -490,7 +477,7 @@ extern "C" int ttb_gemm(const TtbGemmArgs* gp, void* stream) {
     TTB_CHECK_LAUNCH("gemm_ref_kernel");
     return 0;
   }
-  // tile choice: fill the 148 SMs; small-N / small-M problems use narrower tiles
+  // tile choice: fill the SMs; small-N / small-M problems use narrower tiles
   const long long tiles128 = (long long)((g.N + 127) / 128) * ((g.M + BM - 1) / BM) * g.batch;
   if (g.cluster > 1) {
     // thread-block clusters along N sharing the activation tile by TMA multicast (gemm_mc.cuh)
@@ -504,44 +491,37 @@ extern "C" int ttb_gemm(const TtbGemmArgs* gp, void* stream) {
     if (bn == 64) return g.cluster == 4 ? launch_mc<64, 4, 4>(g, ep, st) : launch_mc<64, 4, 2>(g, ep, st);
     return g.cluster == 4 ? launch_mc<128, 3, 4>(g, ep, st) : launch_mc<128, 3, 2>(g, ep, st);
   }
-  if (g.variant == 6) {         // CTA-pair (cta_group::2) kernel: round-2 experiment, see gemm_2cta.cuh
-    if (g.splitk > 1) { set_error("ttb_gemm: the CTA-pair kernel has no split-K"); return -1; }
-    return g.tile_n == 128 ? launch_2cta<128, 6>(g, ep, st) : launch_2cta<256, 6>(g, ep, st);
-  }
-  static int persist = -1;   // TTB_GEMM_PERSIST=0 selects the one-tile-per-CTA kernels (A/B comparison)
-  if (persist < 0) { const char* e = getenv("TTB_GEMM_PERSIST"); persist = e ? atoi(e) : 1; }
-  // Measured on B200 (profiles/op_profile_r01_*): the persistent kernel wins when there are several tiles per SM
-  // (CLVP: 131 -> 90 ms; diffusion qkv conv 66 -> 50 us) and loses on the skinny decode GEMMs (one wave of tiny tiles,
-  // where 2-4 resident CTAs per SM hide latency better than one deep pipeline), so it is used for >= 2 waves only.
+  if (g.variant == 6) { set_error("ttb_gemm: variant 6 (CTA-pair MMA) needs hardware this library does not target"); return -1; }
+  static int persist = -1;   // TTB_GEMM_PERSIST=1 sends problems of >= 2 waves to the persistent kernel (A/B comparison)
+  if (persist < 0) { const char* e = getenv("TTB_GEMM_PERSIST"); persist = e ? atoi(e) : 0; }
+  // Off by default: on H100 (80GB HBM3, 700 W) the one-tile kernels were faster on every stage that has several tiles
+  // per SM (standard preset: CLVP 156 -> 118 ms, diffusion 1061 -> 992 ms): the persistent kernel's consumers do not
+  // overlap a tile's epilogue with the next tile's main loop, which co-resident one-tile CTAs do.
   if (g.variant == 2) {
-    if (g.tile_n == 32) return launch_persistent<32, 8, 4>(g, ep, st);
-    if (g.tile_n == 64) return launch_persistent<64, 8, 4>(g, ep, st);
-    return launch_persistent<128, 6, 4>(g, ep, st);
+    if (g.tile_n == 32) return launch_persistent<32, 8>(g, ep, st);
+    if (g.tile_n == 64) return launch_persistent<64, 6>(g, ep, st);
+    return launch_persistent<128, 4>(g, ep, st);
   }
   const int use_persist = (g.variant == 1) ? 0 : persist;
-  if (use_persist && g.tile_n == 0 && tiles128 >= 2 * 148) return launch_persistent<128, 6, 4>(g, ep, st);
+  if (use_persist && g.tile_n == 0 && tiles128 >= 2 * num_sms()) return launch_persistent<128, 4>(g, ep, st);
   if (use_persist == 2) {        // TTB_GEMM_PERSIST=2: force the persistent kernels everywhere (experiments)
-    if (g.tile_n == 32) return launch_persistent<32, 8, 4>(g, ep, st);
-    if (g.tile_n == 64 || (g.tile_n == 0 && tiles128 < 148)) return launch_persistent<64, 8, 4>(g, ep, st);
-    if (g.tile_n != 256) return launch_persistent<128, 6, 4>(g, ep, st);
+    if (g.tile_n == 32) return launch_persistent<32, 8>(g, ep, st);
+    if (g.tile_n == 64 || (g.tile_n == 0 && tiles128 < num_sms())) return launch_persistent<64, 6>(g, ep, st);
+    if (g.tile_n != 256) return launch_persistent<128, 4>(g, ep, st);
   }
   if (g.tile_n == 32) {
     // the skinny decode GEMMs are latency-bound (k-block time = TMA round trip / stages): 5 stages still allow two
-    // CTAs per SM (2 x 100 KB). TTB_GEMM_T32_STAGES=4 restores the 4-stage kernel for A/B runs; variant 3 forces 5.
+    // CTAs per SM (2 x 101 KB of the 227 KB). TTB_GEMM_T32_STAGES=4 restores the 4-stage kernel for A/B runs; variant 3 forces 5.
     static int t32 = -1;
     if (t32 < 0) { const char* e = getenv("TTB_GEMM_T32_STAGES"); t32 = e ? atoi(e) : 5; }
     return (g.variant == 3 || (g.variant != 4 && t32 == 5)) ? launch_tc<32, 5>(g, ep, st) : launch_tc<32, 4>(g, ep, st);
   }
   // 64-wide tiles, 8 stages, one CTA per SM (variant 3): for skinny problems whose 64-wide grid fits one wave, the deep
-  // pipeline keeps ~190 KB in flight per SM, which is what saturates an SM's inbound path (measured ~150-190 GB/s)
+  // pipeline keeps ~190 KB in flight per SM
   if (g.tile_n == 64 && g.variant == 3) return launch_tc<64, 8>(g, ep, st);
-  if (g.tile_n == 64 || (g.tile_n == 0 && tiles128 < 148)) return launch_tc<64, 4>(g, ep, st);
-  // large problems are L2-bandwidth bound with 128x128 tiles (64 flop/B at ~6.3 KB/clk of L2): 128x256 tiles raise the
-  // intensity to 85 flop/B when the grid still covers most SMs
-  const long long tiles256 = (long long)((g.N + 255) / 256) * ((g.M + BM - 1) / BM) * g.batch;
-  // (measured on B200: 1 CTA/SM with 256-wide tiles is slower than 2 CTAs/SM with 128-wide ones, so only on request)
-  (void)tiles256;
+  if (g.tile_n == 64 || (g.tile_n == 0 && tiles128 < num_sms())) return launch_tc<64, 4>(g, ep, st);
+  // 128x256 tiles (64 vs 85 flop per operand byte) only on request
   if (g.tile_n == 256) return launch_tc<256, 3>(g, ep, st);
-  if (g.variant == 5) return launch_tc<128, 3, true>(g, ep, st);     // two TMA issuers (round-2 experiment)
+  if (g.variant == 5) return launch_tc<128, 3, true>(g, ep, st);     // two TMA issuers (experiment)
   return launch_tc<128, 3>(g, ep, st);
 }

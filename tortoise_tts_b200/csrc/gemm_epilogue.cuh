@@ -1,45 +1,36 @@
-// GEMM epilogue shared by the tcgen05 GEMM kernels (included by gemm.cu after GemmEpilogue is defined).
+// GEMM epilogue shared by the wgmma GEMM kernels (included by gemm.cu after GemmEpilogue is defined).
 //
-// tcgen05.ld hands every thread one accumulator ROW (32 consecutive columns). Writing that row straight to global
-// memory makes each warp-wide store touch 32 different cache lines, so the 32x32 chunk goes through a padded
-// shared-memory tile: 8 lanes then cover one row's 128 bytes and a warp instruction moves 4 complete rows, for the
-// residual read and the fp32 / bf16 writes alike.
-//
-// Measured with ttb_debug_gemm_trace (profiles/gemm_trace_r01.txt): the first version of this epilogue -- one
-// function with every activation and every ragged-edge case behind run-time branches, inside the chunk loop -- took
-// ~2.3 us per 32-column chunk whatever it stored (9-10 us per 128x128 tile against a 5 us mainloop): the executed
-// path was spread over ~39 KB of code, and residual loads serialised behind possibly-aliasing stores. Hence:
+// wgmma leaves the accumulator spread over the registers of the two consumer warpgroups (8 rows x 4 column pairs per
+// warp and instruction fragment). Writing fragments straight to global memory would touch 8 cache lines per store, so
+// the tile first goes, raw, to a padded fp32 tile in shared memory (gemm_stage_accumulator); the epilogue then reads it
+// back row-wise: 8 lanes cover one row's 128 bytes and a warp instruction moves 4 complete rows, for the residual read
+// and the fp32 / bf16 writes alike. Each warp finishes one 32-row block, the two warps of a block alternate 32-column
+// chunks.
 //   * the activation is a template parameter and the run-time switch sits OUTSIDE the chunk loop;
-//   * a chunk that is complete (32 rows, 32 columns, 16-byte aligned rows) takes a branch-free FAST path of ~100
-//     instructions; ragged edges take a separate, simple per-row SLOW path;
+//   * a chunk that is complete (32 columns, 16-byte aligned rows) takes a branch-free FAST path; ragged edges take a
+//     separate, simple per-row SLOW path (lane = row);
 //   * the residual (which may alias the output: x += f(x) in place) is loaded for the whole chunk before any store;
-//   * the transpose tile uses a 36-float pitch so both sides are conflict-free 128-bit shared accesses.
+//   * the tile pitch is BN + 8 floats, so both the fragment stores and the row reads are conflict-free.
 #pragma once
 
 namespace ttb {
 
-constexpr int EPI_PITCH = 36;                           // floats per scratch row (144 B: 16-B aligned, conflict-free v4)
-constexpr int EPI_SCRATCH_BYTES = 32 * EPI_PITCH * 4;   // per epilogue warp
-
-TTB_DEVINL void sts128(uint32_t addr, float a, float b, float c, float d) {
-  asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
 TTB_DEVINL float4 lds128(uint32_t addr) {
   float4 v;
   asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
   return v;
 }
 
-// tcgen05.wait::ld that also carries a data dependency on the loaded registers, so that no use of r[] can be scheduled
-// above the wait.
-TTB_DEVINL void tmem_ld_wait_dep(uint32_t* r) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                 "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]),
-                 "+r"(r[16]), "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]), "+r"(r[23]),
-                 "+r"(r[24]), "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]), "+r"(r[30]), "+r"(r[31])
-               :
-               : "memory");
+// Accumulator fragments of this thread (rows 64 wg + 16 w + l/4 (+8), see common.cuh) -> fp32 tile [128][BN + 8].
+template <int BN>
+TTB_DEVINL void gemm_stage_accumulator(const float* acc, uint32_t tile, int cwarp, int lane) {
+  constexpr int PITCH = BN + 8;
+  const uint32_t base = tile + (uint32_t)((cwarp * 16 + (lane >> 2)) * PITCH + 2 * (lane & 3)) * 4;
+#pragma unroll
+  for (int i = 0; i < BN / 2; i += 4) {
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(base + (uint32_t)(2 * i) * 4), "f"(acc[i]), "f"(acc[i + 1]) : "memory");
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(base + (uint32_t)(8 * PITCH + 2 * i) * 4), "f"(acc[i + 2]), "f"(acc[i + 3]) : "memory");
+  }
 }
 
 template <int ACT>
@@ -79,50 +70,31 @@ TTB_DEVINL void epi_gn_store(float gs, float gq, int nb, int m_base, int lane, l
 
 // ---- FAST path: all 32 columns exist, everything aligned. Branch-free apart from the uniform pointer tests. Only the
 // first `rows_valid` (1..32) of the 32 rows exist (< 32: the last row block of a ragged M): the row-wise residual loads
-// and stores are predicated per row -- one code path, so the kernels' register allocation and code size stay as they were. (The per-lane scalar SLOW path costs ~18 us for such a block -- profiles/gemm_trace_r01_fine.txt,
-// "SM 77" -- and with M = 1872 = 14.6 tiles it sat on the tail of every denoiser GEMM.)
+// and stores are predicated per row. `blk` = shared-memory address of (first row of the block, first column of the
+// chunk) in the staged accumulator tile, `pitch` in floats.
 template <int ACT>
-TTB_DEVINL void epi_chunk_fast(const uint32_t* r, int nb, int m_base, int rows_valid, int lane, long long bz,
-                               const GemmEpilogue& ep, uint32_t scratch) {
-  const uint32_t wrow = scratch + (uint32_t)lane * (EPI_PITCH * 4);
+TTB_DEVINL void epi_chunk_fast(uint32_t blk, int pitch, int nb, int m_base, int rows_valid, int lane, long long bz,
+                               const GemmEpilogue& ep) {
   const bool GN = ep.gn_part != nullptr;
-  float v[32];
-  if (ep.bias) {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float4 b = __ldg(reinterpret_cast<const float4*>(ep.bias + nb) + j);
-      v[4 * j] = fmaf(__uint_as_float(r[4 * j]), ep.alpha, b.x);
-      v[4 * j + 1] = fmaf(__uint_as_float(r[4 * j + 1]), ep.alpha, b.y);
-      v[4 * j + 2] = fmaf(__uint_as_float(r[4 * j + 2]), ep.alpha, b.z);
-      v[4 * j + 3] = fmaf(__uint_as_float(r[4 * j + 3]), ep.alpha, b.w);
-    }
-  } else {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]) * ep.alpha;
-  }
+  const int rr0 = lane >> 3, c = (lane & 7) * 4;     // 4 rows per instruction: 8 lanes x 4 columns per row
+  float4 b = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (ep.bias) b = __ldg(reinterpret_cast<const float4*>(ep.bias + nb + c));
   if (ACT == TTB_ACT_GEGLU) {
-    // columns interleaved (u0,g0,u1,g1,...): out[j] = u * gelu_erf(g); output width N/2 -> 16 columns per chunk
+    // columns interleaved (u0,g0,u1,g1,...): out[j] = u * gelu_erf(g); output width N/2 -> 2 columns per lane
+    const long long col = (nb >> 1) + (c >> 1);
 #pragma unroll
-    for (int k = 0; k < 4; ++k)
-      sts128(wrow + k * 16, v[8 * k] * gelu_erf(v[8 * k + 1]), v[8 * k + 2] * gelu_erf(v[8 * k + 3]),
-             v[8 * k + 4] * gelu_erf(v[8 * k + 5]), v[8 * k + 6] * gelu_erf(v[8 * k + 7]));
-    __syncwarp();
-    const int rr0 = lane >> 2, c = (lane & 3) * 4;   // 8 rows per instruction: 4 lanes x 4 columns per row
-    const long long col = (nb >> 1) + c;
-#pragma unroll
-    for (int it = 0; it < 4; ++it) {
-      const int rr = it * 8 + rr0;
-      const float4 o = lds128(scratch + (uint32_t)(rr * EPI_PITCH + c) * 4);
+    for (int it = 0; it < 8; ++it) {
+      const int rr = it * 4 + rr0;
+      const float4 a = lds128(blk + (uint32_t)(rr * pitch + c) * 4);
+      const float o0 = fmaf(a.x, ep.alpha, b.x) * gelu_erf(fmaf(a.y, ep.alpha, b.y));
+      const float o1 = fmaf(a.z, ep.alpha, b.z) * gelu_erf(fmaf(a.w, ep.alpha, b.w));
       const long long m = m_base + rr;
       if (rr >= rows_valid) continue;
-      if (ep.out_bf16)
-        *reinterpret_cast<uint2*>(ep.out_bf16 + bz * ep.outb_bstride + m * ep.ldob + col) = make_uint2(pack_bf16(o.x, o.y), pack_bf16(o.z, o.w));
-      if (ep.out_f32) *reinterpret_cast<float4*>(ep.out_f32 + bz * ep.outf_bstride + m * ep.ldo + col) = o;
+      if (ep.out_bf16) *reinterpret_cast<uint32_t*>(ep.out_bf16 + bz * ep.outb_bstride + m * ep.ldob + col) = pack_bf16(o0, o1);
+      if (ep.out_f32) *reinterpret_cast<float2*>(ep.out_f32 + bz * ep.outf_bstride + m * ep.ldo + col) = make_float2(o0, o1);
     }
-    __syncwarp();                                    // scratch is reused by the next chunk
     return;
   }
-  const int rr0 = lane >> 3, c = (lane & 7) * 4;     // 4 rows per instruction: 8 lanes x 4 columns per row
   const long long col = nb + c;
   // residual for the positions this lane stores, all issued before the first store
   float4 rs[8];
@@ -134,16 +106,16 @@ TTB_DEVINL void epi_chunk_fast(const uint32_t* r, int nb, int m_base, int rows_v
       else rs[it] = make_float4(0.f, 0.f, 0.f, 0.f);
     }
   }
-#pragma unroll
-  for (int k = 0; k < 8; ++k)
-    sts128(wrow + k * 16, epi_act<ACT>(v[4 * k]), epi_act<ACT>(v[4 * k + 1]), epi_act<ACT>(v[4 * k + 2]),
-           epi_act<ACT>(v[4 * k + 3]));
-  __syncwarp();
   float gs = 0.f, gq = 0.f;                          // GroupNorm partial of this 32 x 32 block (ep.gn_part)
 #pragma unroll
   for (int it = 0; it < 8; ++it) {
     const int rr = it * 4 + rr0;
-    float4 o = lds128(scratch + (uint32_t)(rr * EPI_PITCH + c) * 4);
+    const float4 a = lds128(blk + (uint32_t)(rr * pitch + c) * 4);
+    float4 o;
+    o.x = epi_act<ACT>(fmaf(a.x, ep.alpha, b.x));
+    o.y = epi_act<ACT>(fmaf(a.y, ep.alpha, b.y));
+    o.z = epi_act<ACT>(fmaf(a.z, ep.alpha, b.z));
+    o.w = epi_act<ACT>(fmaf(a.w, ep.alpha, b.w));
     if (ep.residual) { o.x += rs[it].x; o.y += rs[it].y; o.z += rs[it].z; o.w += rs[it].w; }
     const long long m = m_base + rr;
     if (rr >= rows_valid) continue;
@@ -156,7 +128,6 @@ TTB_DEVINL void epi_chunk_fast(const uint32_t* r, int nb, int m_base, int rows_v
     }
   }
   if (GN) epi_gn_store(gs, gq, nb, m_base, lane, bz, ep);
-  __syncwarp();                                      // scratch is reused by the next chunk
 }
 
 // ---- SLOW path (ragged M / N edges, unaligned rows): each lane finishes its own accumulator row with scalar accesses.
@@ -198,28 +169,30 @@ TTB_DEVINL void epi_chunk_slow(const uint32_t* r, int nb, int N, int m, int M, l
   }
 }
 
-// Whole accumulator tile of one epilogue warp: taddr = TMEM address of (lane group, first column). When release_bar
-// is given it is arrived on once the last tcgen05.ld has completed (persistent kernel: the MMA warp may then overwrite
-// this accumulator buffer while the stores are still going out).
+// One 32-row block of the staged accumulator tile, finished by one warp: `blk` = shared-memory address of the block's
+// first row, chunks ch_begin, ch_begin + ch_step, ... of 32 columns.
 template <int BN, int ACT>
-TTB_DEVINL void gemm_epilogue_tile(uint32_t taddr, int n0, int N, int m_base, int M, int lane, long long bz,
-                                   const GemmEpilogue& ep, uint32_t scratch, uint64_t* release_bar) {
+TTB_DEVINL void gemm_epilogue_tile(uint32_t blk, int n0, int N, int m_base, int M, int lane, long long bz,
+                                   const GemmEpilogue& ep, int ch_begin, int ch_step) {
   constexpr int NCH = BN / 32;
+  constexpr int PITCH = BN + 8;
   const bool aligned = epi_flags(ep).aligned;
   const int rows_valid = min(32, M - m_base);        // warp-uniform; <= 0: this warp's rows are all past M
-  // rolled on purpose: one chunk's worth of code and registers (the 128-wide kernel must stay <= 168 registers for
-  // two CTAs per SM); the co-resident warps cover the tcgen05.ld latency
+  // rolled on purpose: one chunk's worth of code and registers
 #pragma unroll 1
-  for (int ch = 0; ch < NCH; ++ch) {
+  for (int ch = ch_begin; ch < NCH; ch += ch_step) {
     const int nb = n0 + ch * 32;
-    uint32_t r[32];
-    tmem_ld_32x32b_x32(taddr + (uint32_t)ch * 32, r);
-    tmem_ld_wait_dep(r);
-    if (release_bar && ch == NCH - 1) { tc_fence_before(); mbar_arrive(release_bar); }
     if (nb >= N || rows_valid <= 0) continue;        // warp-uniform
     if (aligned && nb + 32 <= N) {
-      epi_chunk_fast<ACT>(r, nb, m_base, rows_valid, lane, bz, ep, scratch);
+      epi_chunk_fast<ACT>(blk + (uint32_t)ch * 128, PITCH, nb, m_base, rows_valid, lane, bz, ep);
     } else {
+      uint32_t r[32];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float4 a = lds128(blk + (uint32_t)(lane * PITCH + ch * 32 + 4 * j) * 4);
+        r[4 * j] = __float_as_uint(a.x); r[4 * j + 1] = __float_as_uint(a.y);
+        r[4 * j + 2] = __float_as_uint(a.z); r[4 * j + 3] = __float_as_uint(a.w);
+      }
       float gs = 0.f, gq = 0.f;                      // rows past M contribute nothing
       epi_chunk_slow<ACT>(r, nb, N, m_base + lane, M, bz, ep, gs, gq);
       if (ep.gn_part) epi_gn_store(gs, gq, nb, m_base, lane, bz, ep);
@@ -228,15 +201,15 @@ TTB_DEVINL void gemm_epilogue_tile(uint32_t taddr, int n0, int N, int m_base, in
 }
 
 template <int BN>
-TTB_DEVINL void gemm_epilogue_dispatch(uint32_t taddr, int n0, int N, int m_base, int M, int lane, long long bz,
-                                       const GemmEpilogue& ep, uint32_t scratch, uint64_t* release_bar) {
+TTB_DEVINL void gemm_epilogue_dispatch(uint32_t blk, int n0, int N, int m_base, int M, int lane, long long bz,
+                                       const GemmEpilogue& ep, int ch_begin, int ch_step) {
   switch (ep.act) {
-    case TTB_ACT_GEGLU: gemm_epilogue_tile<BN, TTB_ACT_GEGLU>(taddr, n0, N, m_base, M, lane, bz, ep, scratch, release_bar); break;
-    case TTB_ACT_GELU_NEW: gemm_epilogue_tile<BN, TTB_ACT_GELU_NEW>(taddr, n0, N, m_base, M, lane, bz, ep, scratch, release_bar); break;
-    case TTB_ACT_SILU: gemm_epilogue_tile<BN, TTB_ACT_SILU>(taddr, n0, N, m_base, M, lane, bz, ep, scratch, release_bar); break;
-    case TTB_ACT_LRELU02: gemm_epilogue_tile<BN, TTB_ACT_LRELU02>(taddr, n0, N, m_base, M, lane, bz, ep, scratch, release_bar); break;
-    case TTB_ACT_TANH: gemm_epilogue_tile<BN, TTB_ACT_TANH>(taddr, n0, N, m_base, M, lane, bz, ep, scratch, release_bar); break;
-    default: gemm_epilogue_tile<BN, TTB_ACT_NONE>(taddr, n0, N, m_base, M, lane, bz, ep, scratch, release_bar); break;
+    case TTB_ACT_GEGLU: gemm_epilogue_tile<BN, TTB_ACT_GEGLU>(blk, n0, N, m_base, M, lane, bz, ep, ch_begin, ch_step); break;
+    case TTB_ACT_GELU_NEW: gemm_epilogue_tile<BN, TTB_ACT_GELU_NEW>(blk, n0, N, m_base, M, lane, bz, ep, ch_begin, ch_step); break;
+    case TTB_ACT_SILU: gemm_epilogue_tile<BN, TTB_ACT_SILU>(blk, n0, N, m_base, M, lane, bz, ep, ch_begin, ch_step); break;
+    case TTB_ACT_LRELU02: gemm_epilogue_tile<BN, TTB_ACT_LRELU02>(blk, n0, N, m_base, M, lane, bz, ep, ch_begin, ch_step); break;
+    case TTB_ACT_TANH: gemm_epilogue_tile<BN, TTB_ACT_TANH>(blk, n0, N, m_base, M, lane, bz, ep, ch_begin, ch_step); break;
+    default: gemm_epilogue_tile<BN, TTB_ACT_NONE>(blk, n0, N, m_base, M, lane, bz, ep, ch_begin, ch_step); break;
   }
 }
 

@@ -1,16 +1,15 @@
-// Cluster / TMA-multicast variant of the tcgen05 GEMM (included by gemm.cu).
+// Cluster / TMA-multicast variant of the wgmma GEMM (included by gemm.cu).
 //
-// Motivation (measured, profiles/ncu_summary_r01_run10.txt + DESIGN.md §9): with one CTA per 128xBN tile every CTA pulls
-// its own copy of the 128x64 activation tile per k-block, and the L2->SM fabric (~6.3 KB/clk chip-wide) saturates long
-// before the tensor pipe does (decode GEMMs with BN=32 move 16 KB of A for 4 KB of weights per k-block).
+// With one CTA per 128xBN tile every CTA pulls its own copy of the 128x64 activation tile per k-block, and the L2->SM
+// fabric saturates before the tensor pipe does (decode GEMMs with BN=32 move 16 KB of A for 4 KB of weights per k-block).
 // Here CL CTAs that are neighbours along N (same m-tile) form a thread-block cluster: each loads 1/CL of the A tile
 // and MULTICASTS it into the shared memory of all CL CTAs (cp.async.bulk.tensor ... .multicast::cluster); the weight
 // tile stays private. Per k-block a CTA reads 16/CL KB + B instead of 16 KB + B.
 //
 // Synchronisation: every CTA arms its own full barrier with the whole stage's bytes (its B tile + CL multicast slices of
 // A land in ITS smem and complete_tx on ITS barrier). A stage may only be overwritten when ALL CTAs of the cluster have
-// consumed it, so the MMA thread's tcgen05.commit arrives (multicast) on the empty barrier of every CTA in the cluster
-// and empty barriers are initialised with count CL.
+// consumed it, so each consumer warpgroup arrives on the empty barrier of every CTA in the cluster once its wgmma group
+// has retired, and empty barriers are initialised with count 2 * CL.
 #pragma once
 
 namespace ttb {
@@ -31,9 +30,13 @@ TTB_DEVINL void tma_load_3d_mc(void* smem_dst, const CUtensorMap* map, uint64_t*
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "h"(mask), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
-TTB_DEVINL void umma_commit_mc(uint64_t* bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"(mask) : "memory");
+// arrive on the copy of `bar` in CTA `cta` of this cluster
+TTB_DEVINL void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+  asm volatile(
+      "{\n\t.reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}\n" ::"r"(smem_u32(bar)), "r"(cta)
+      : "memory");
 }
 
 template <int BN, int STAGES, int CL>
@@ -48,8 +51,6 @@ gemm_bf16_tc_mc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_c
   constexpr uint16_t MASK = (uint16_t)((1u << CL) - 1);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* accum_bar = empty_bar + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_bar + 1);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -62,22 +63,16 @@ gemm_bf16_tc_mc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_c
   const int kb_begin = kb_per_split > 0 ? bz * kb_per_split : 0;
   const int num_kb = kb_per_split > 0 ? min(kb_per_split, kb_total - kb_begin) : kb_total;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == PRODUCER_WARP && lane == 0) {
     tma_prefetch_desc(&map_a);
     tma_prefetch_desc(&map_b);
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], CL); }
-    mbar_init(accum_bar, 1);
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2 * CL); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<BN>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  __syncwarp();
   cluster_sync_all();            // peers' barriers are initialised before anyone multicasts into them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == PRODUCER_WARP) {
     if (lane == 0) {
       int stage = 0; uint32_t phase = 0;
       for (int kbi = 0; kbi < num_kb; ++kbi) {
@@ -95,40 +90,26 @@ gemm_bf16_tc_mc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_c
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_bf16(BM, BN, 0, 0);
-      int stage = 0; uint32_t phase = 0;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint32_t sa = smem_u32(smem + stage * L::STAGE_BYTES);
-        const uint32_t sb = sa + L::A_BYTES;
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k)
-          umma_bf16_ss(tmem_base, umma_desc_kmajor_sw128(sa + k * 32), umma_desc_kmajor_sw128(sb + k * 32), idesc,
-                       (kb | k) != 0 ? 1u : 0u);
-        umma_commit_mc(&empty_bar[stage], MASK);      // release the stage in every CTA of the cluster
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      umma_commit(accum_bar);
-    }
+    __syncwarp();
   } else {
-    const int q = warp & 3;
-    mbar_wait(accum_bar, 0);
-    tc_fence_after();
-    // the pipeline stages are idle by now and serve as the transpose scratch
-    gemm_epilogue_dispatch<BN>(tmem_base + ((uint32_t)(q * 32) << 16), n0, N, m0 + q * 32, M, lane, (long long)bz, ep,
-                               smem_u32(smem + (warp - 2) * EPI_SCRATCH_BYTES), nullptr);
-    tc_fence_before();
+    const int wg = warp >> 2;
+    const int rb = warp >> 1;
+    float acc[BN / 2];
+    int stage = 0; uint32_t phase = 0;
+    gemm_consumer_mainloop<BN, STAGES>(acc, smem, L::STAGE_BYTES, L::A_BYTES, full_bar, empty_bar, num_kb, stage, phase, wg,
+                                       (threadIdx.x & 127) == 0, [](uint64_t* b) {
+                                         for (uint32_t c = 0; c < (uint32_t)CL; ++c) mbar_arrive_cluster(b, c);   // release the stage in every CTA
+                                       });
+    // every wgmma of both warpgroups has retired and every multicast slice of this CTA's stages has landed: the pipeline
+    // stages are idle and take the staged accumulator tile
+    named_barrier(1, GEMM_CONSUMERS);
+    gemm_stage_accumulator<BN>(acc, smem_u32(smem), warp, lane);
+    named_barrier(1, GEMM_CONSUMERS);
+    gemm_epilogue_dispatch<BN>(smem_u32(smem) + (uint32_t)(rb * 32 * (BN + 8)) * 4, n0, N, m0 + rb * 32, M, lane, (long long)bz,
+                               ep, warp & 1, 2);
   }
   __syncthreads();
-  __syncwarp();
-  cluster_sync_all();            // nobody exits while a peer may still multicast into / arrive on its shared memory
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<BN>(tmem_base);
-  }
+  cluster_sync_all();            // nobody exits while a peer may still arrive on its barriers
 }
 
 template <int BN, int STAGES, int CL>

@@ -1,42 +1,35 @@
-// Persistent variant of the tcgen05 GEMM (included by gemm.cu after GemmEpilogue / BM / BK are defined).
+// Persistent variant of the wgmma GEMM (included by gemm.cu after GemmEpilogue / BM / BK are defined).
 //
 // One CTA per SM loops over output tiles (tile id -> m fastest, then n, then batch/split), so that
-//   * the TMA -> MMA pipeline (PSTAGES deep) never drains between tiles,
-//   * the accumulator is double-buffered in TMEM (2 x BN columns): the epilogue of tile t overlaps the MMAs of t+1,
-//   * barrier init / TMEM allocation / descriptor prefetch are paid once per CTA instead of once per tile.
-// Roles: warp 0 = TMA producer, warp 1 = MMA issuer (+ TMEM alloc), warps 2..2+EW-1 = epilogue. With EW = 8 two warps
-// share each TMEM lane quarter and split the tile's columns: measured (profiles/gemm_trace_r01.txt) a 4-warp epilogue
-// needs ~4.9 us per 128x128 tile while the mainloop alone needs ~2.5 us, so with 4 warps the epilogue, not the tensor
-// pipe, set the pace of the persistent loop.
+//   * the TMA producer runs ahead into the next tile's k-blocks while the consumers finish the epilogue of this one,
+//   * barrier init / descriptor prefetch are paid once per CTA instead of once per tile.
+// Roles: warps 0..7 = two consumer warpgroups (wgmma, then the epilogue of their own 64 rows from a dedicated staging
+// tile), warp 8 = TMA producer.
 #pragma once
 
 namespace ttb {
 
-template <int BN, int PSTAGES, int EW>
+template <int BN, int PSTAGES>
 struct GemmPSmem {
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int BAR_OFF = PSTAGES * STAGE_BYTES;
-  static constexpr int SCRATCH_OFF = BAR_OFF + (2 * PSTAGES + 4) * 8 + 16;   // EW epilogue warps x transpose tile
-  static constexpr int TOTAL = SCRATCH_OFF + EW * EPI_SCRATCH_BYTES + 1024;
+  static constexpr int ACC_OFF = PSTAGES * STAGE_BYTES;                      // staged accumulator tile [128][BN + 8] fp32
+  static constexpr int BAR_OFF = ACC_OFF + BM * (BN + 8) * 4;
+  static constexpr int TOTAL = BAR_OFF + 2 * PSTAGES * 8 + 16 + 1024;
   static_assert(TOTAL <= 227 * 1024, "persistent GEMM shared memory");
 };
 
-template <int BN, int PSTAGES, int EW>
-__global__ void __launch_bounds__(64 + 32 * EW, 1)
+template <int BN, int PSTAGES>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_tc_persistent_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                                int M, int N, int K, int taps, int pad, int a_batch_mul, int kb_per_split, int m_tiles,
                                int n_tiles, int z_tiles, GemmEpilogue ep) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  using L = GemmPSmem<BN, PSTAGES, EW>;
-  static_assert(EW == 4 || (EW == 8 && BN >= 64), "epilogue warps");
+  using L = GemmPSmem<BN, PSTAGES>;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);
   uint64_t* empty_bar = full_bar + PSTAGES;
-  uint64_t* acc_full = empty_bar + PSTAGES;     // [2] MMA -> epilogue
-  uint64_t* acc_empty = acc_full + 2;           // [2] epilogue -> MMA
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -44,21 +37,16 @@ gemm_bf16_tc_persistent_kernel(const __grid_constant__ CUtensorMap map_a, const 
   const int kb_total = kblocks_per_tap * taps;
   const int total_tiles = m_tiles * n_tiles * z_tiles;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == PRODUCER_WARP && lane == 0) {
     tma_prefetch_desc(&map_a);
     tma_prefetch_desc(&map_b);
-    for (int s = 0; s < PSTAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&acc_full[s], 1); mbar_init(&acc_empty[s], 32 * EW); }
+    for (int s = 0; s < PSTAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<2 * BN>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();
 
-  if (warp == 0) {
+  if (warp == PRODUCER_WARP) {
     if (lane == 0) {
       int stage = 0; uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
@@ -81,58 +69,29 @@ gemm_bf16_tc_persistent_kernel(const __grid_constant__ CUtensorMap map_a, const 
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_bf16(BM, BN, 0, 0);
-      int stage = 0; uint32_t phase = 0;
-      int t = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++t) {
-        const int bz = tile / (m_tiles * n_tiles);
-        const int kb_begin = kb_per_split > 0 ? bz * kb_per_split : 0;
-        const int num_kb = kb_per_split > 0 ? min(kb_per_split, kb_total - kb_begin) : kb_total;
-        const int acc = t & 1;
-        mbar_wait(&acc_empty[acc], ((t >> 1) & 1) ^ 1);     // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)(acc * BN);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * L::STAGE_BYTES);
-          const uint32_t sb = sa + L::A_BYTES;
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k)
-            umma_bf16_ss(tmem_d, umma_desc_kmajor_sw128(sa + k * 32), umma_desc_kmajor_sw128(sb + k * 32), idesc,
-                         (kb | k) != 0 ? 1u : 0u);
-          umma_commit(&empty_bar[stage]);
-          if (++stage == PSTAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&acc_full[acc]);
-      }
-    }
+    __syncwarp();
   } else {
-    const int q = warp & 3;
-    int t = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++t) {
+    const int wg = warp >> 2;
+    const int rb = warp >> 1;
+    const uint32_t acc_tile = smem_u32(smem + L::ACC_OFF);
+    int stage = 0; uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const int mt = tile % m_tiles, rest = tile / m_tiles;
       const int nt = rest % n_tiles, bz = rest / n_tiles;
-      const int n0 = nt * BN;
-      const int acc = t & 1;
-      mbar_wait(&acc_full[acc], (t >> 1) & 1);
-      tc_fence_after();
-      // the accumulator buffer is handed back to the MMA warp as soon as its last tcgen05.ld has completed
-      constexpr int BNW = BN / (EW / 4);               // columns per epilogue warp
-      const int cg = (warp - 2) >> 2;                  // column group of this warp (0 when EW == 4)
-      gemm_epilogue_dispatch<BNW>(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * BN + cg * BNW), n0 + cg * BNW, N,
-                                  mt * BM + q * 32, M, lane, (long long)bz, ep,
-                                  smem_u32(smem + L::SCRATCH_OFF + (warp - 2) * EPI_SCRATCH_BYTES), &acc_empty[acc]);
+      const int kb_begin = kb_per_split > 0 ? bz * kb_per_split : 0;
+      const int num_kb = kb_per_split > 0 ? min(kb_per_split, kb_total - kb_begin) : kb_total;
+      float acc[BN / 2];
+      gemm_consumer_mainloop<BN, PSTAGES>(acc, smem, L::STAGE_BYTES, L::A_BYTES, full_bar, empty_bar, num_kb, stage, phase, wg,
+                                          (threadIdx.x & 127) == 0, [](uint64_t* b) { mbar_arrive(b); });
+      // rows [64 wg, 64 wg + 64) of the staging tile are written and read by warpgroup wg only
+      named_barrier(1 + wg, 128);                      // the previous tile's readers are done
+      gemm_stage_accumulator<BN>(acc, acc_tile, warp, lane);
+      named_barrier(1 + wg, 128);
+      gemm_epilogue_dispatch<BN>(acc_tile + (uint32_t)(rb * 32 * (BN + 8)) * 4, nt * BN, N, mt * BM + rb * 32, M, lane,
+                                 (long long)bz, ep, warp & 1, 2);
     }
   }
   pdl_launch_dependents();      // tail trigger (see gemm.cu)
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<2 * BN>(tmem_base);
-  }
 }
 
 }  // namespace ttb

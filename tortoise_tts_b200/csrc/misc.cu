@@ -181,8 +181,8 @@ diffusion_step_kernel(TtbDiffStepArgs a) {
 __global__ void counter_add_kernel(int* c, int d) { *c += d; }
 
 // ------------------------------------------------------------------ CFG pair: exchange of the two denoiser branches
-// Two GPUs evaluate one classifier-free-guidance branch each (diffusion_engine.py). Round 1 exchanged the [S, 200] fp32
-// outputs with an eager NCCL all-gather between two CUDA graphs per step (2.55 ms per step against 1.9 ms of compute).
+// Two GPUs evaluate one classifier-free-guidance branch each (diffusion_engine.py). The fallback exchanges the [S, 200] fp32
+// outputs with an eager NCCL all-gather between two CUDA graphs per step, which costs more than the step's compute.
 // This kernel is the exchange as ONE graph-capturable launch over peer memory (CUDA IPC mapping of the partner's buffer,
 // NVLink stores): copy my branch into slot (step parity, my branch) of BOTH exchange areas, publish a flag in the
 // partner's memory, wait for the partner's flag. Slots are double-buffered by step parity: the partner can be at most one

@@ -1,5 +1,5 @@
 // Normalisation kernels (HBM/L2-bound): LayerNorm (single or chained), RMSNorm, GroupNorm32 with the fused
-// scale-shift / SiLU consumers. fp32 statistics via warp-shuffle reductions; outputs feed the tcgen05 GEMM as bf16.
+// scale-shift / SiLU consumers. fp32 statistics via warp-shuffle reductions; outputs feed the wgmma GEMM as bf16.
 #include "common.cuh"
 #include "ttb_internal.h"
 
@@ -74,8 +74,7 @@ layernorm_kernel(const float* x, int D, const float* __restrict__ g1, const floa
 
 // One WARP per row (D = 128 * NV, NV <= 8): the row lives in NV float4 per lane, both statistics are xor-shuffle trees,
 // no shared memory and no block barrier. The GPT-2 decode step runs 61 of these on 256 rows between skinny GEMMs
-// (profiles/ncu_launches_r01_ar_decode_step.txt: 11.5 % of the step with the block-per-row kernel above, whose two
-// block_sum round trips dominate a 4 KB row). Same arithmetic as layernorm_kernel (two-pass variance, fixed
+// (the two block_sum round trips of the block-per-row kernel above dominate a 4 KB row). Same arithmetic as layernorm_kernel (two-pass variance, fixed
 // summation order of the split-K partials), only the reduction tree differs.
 
 template <int NV>
@@ -249,9 +248,7 @@ gn_apply_kernel(const float* __restrict__ x, int S, int C, int groups, int cpg, 
 
 // ---------------------------------------------------------------------------------------------------------------
 // Row-wise GroupNorm (the path the denoiser takes: C = 1024, 32 groups). The two kernels above walk one GROUP at a
-// time (128-byte segments 4 KB apart) and re-derive every per-channel constant for each float4; the ncu launch list
-// of a denoiser step (profiles/ncu_launches_r01_diffusion_step.txt) had them at 9.7 + 13.6 us per GroupNorm, i.e.
-// 1.6 TB/s on 15 MB, and 23 % of the step. Here a block owns whole ROWS (4 KB contiguous), thread t owns the float4
+// time (128-byte segments 4 KB apart) and re-derive every per-channel constant for each float4. Here a block owns whole ROWS (4 KB contiguous), thread t owns the float4
 // column t of every row of its block:
 //   stats: per-thread (sum, sumsq) over the block's rows, xor-shuffle over the cpg/4 lanes of a group, then a fixed-order
 //          sum over the block's row lanes in shared memory: one partial per (batch, group, block). No atomics anywhere:
@@ -379,7 +376,7 @@ using namespace ttb;
 // warp-per-row LayerNorm when the row is NV x 128 floats and everything is 16-byte aligned; false = not applicable
 static int gn_early() {
   static int v = -1;
-  if (v < 0) { const char* e = getenv("TTB_GN_EARLY"); v = (e && e[0] == '0') ? 0 : 1; }     // default on: diffusion 625 -> 618 ms
+  if (v < 0) { const char* e = getenv("TTB_GN_EARLY"); v = (e && e[0] == '0') ? 0 : 1; }     // default on
   return v;
 }
 

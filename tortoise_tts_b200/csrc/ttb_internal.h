@@ -8,12 +8,9 @@
 #define TTB_GN_SPLITS TTB_GROUPNORM_SPLITS   // row blocks of the GroupNorm statistics pass (include/ttb.h)
 
 namespace ttb {
-// flash_attn.cu: tcgen05 attention for the large shapes
+// flash_attn.cu: wgmma attention for the large shapes
 bool flash_attention_supported(const TtbAttnArgs& a);
 int flash_attention_launch(const TtbAttnArgs& a, cudaStream_t st);
-// flash_attn2.cu: two query tiles per CTA in ping-pong (large T, packed qkv)
-bool flash_attention2_supported(const TtbAttnArgs& a);
-int flash_attention2_launch(const TtbAttnArgs& a, cudaStream_t st);
 // gemm.cu
 int get_tensor_map_bf16(CUtensorMap* out, const void* ptr, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t stride1_elems,
                         uint64_t stride2_elems, uint32_t b0, uint32_t b1);

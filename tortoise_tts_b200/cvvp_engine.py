@@ -1,4 +1,4 @@
-"""CVVP re-ranker on the sm_100a kernels (SURVEY §8f row 4: `tts(cvvp_amount > 0, voice_samples=...)`).
+"""CVVP re-ranker on the sm_90a kernels (SURVEY §8f row 4: `tts(cvvp_amount > 0, voice_samples=...)`).
 
 Mirrors `CVVP.forward(mel_cond, mel_codes, return_loss=False)` (tortoise/models/cvvp.py:108-124) as `tortoise/api.py:464-468`
 accumulates it: the similarity of every candidate's mel codes to each conditioning clip, averaged over the clips. The

@@ -1,9 +1,9 @@
-"""DiffusionTts denoiser + SpacedDiffusion sampling loop on the sm_100a kernels (hot loop 2, SURVEY §8 rows a9-a12).
+"""DiffusionTts denoiser + SpacedDiffusion sampling loop on the sm_90a kernels (hot loop 2, SURVEY §8 rows a9-a12).
 
 Mirrors `do_spectrogram_diffusion` (tortoise/api.py:117-130): `timestep_independent` once, then `iters` steps of
 p_sample with the conditional and unconditional forward batched as B=2 (the reference runs them sequentially,
 utils/diffusion.py:340-342), scheduler tables resident on the device and the whole step captured in one CUDA graph.
-Activations are token-major [B, S, C]; convolutions are tcgen05 GEMMs (k=3 as three shifted TMA loads).
+Activations are token-major [B, S, C]; convolutions are wgmma GEMMs (k=3 as three shifted TMA loads).
 """
 import math
 
@@ -167,7 +167,7 @@ class DiffusionEngine:
         # the two CFG branches as two kernel chains on two streams instead of one batched pass (see _forward)
         self.CHAINS = int(os.environ.get("TTB_DIFF_CHAINS", "0"))
         # the C x C GEMMs of a step put their first weight tiles into the pipeline ahead of griddepcontrol.wait
-        # (TtbGemmArgs.w_static; the GroupNorm in front of them releases its dependents early): 618 -> 616 ms, TTB_DIFF_WSTATIC=0 = off
+        # (TtbGemmArgs.w_static; the GroupNorm in front of them releases its dependents early); TTB_DIFF_WSTATIC=0 = off
         self.WS = bool(int(os.environ.get("TTB_DIFF_WSTATIC", "1")))
 
     # ------------------------------------------------------------------ building blocks on [B, S, C] fp32 (in place)
@@ -426,8 +426,8 @@ class DiffusionEngine:
         trace = []
 
         # The CUDA graph holds the denoiser evaluation (+ the scheduler epilogue when both CFG branches are local).
-        # In pair mode the NCCL all-gather is NOT captured (a capture attempt of torch.distributed collectives dead-locked
-        # on the GPU box in round 1): graph(forward of my branch) -> eager all-gather -> eager epilogue, per step.
+        # In pair mode the NCCL all-gather is NOT captured (a capture attempt of torch.distributed collectives dead-locks):
+        # graph(forward of my branch) -> eager all-gather -> eager epilogue, per step.
         fused_epilogue = pair is None or st.get("xch") is not None      # the exchange itself is capturable
         if st.get("xch") is not None:
             st["xch"].new_sample()

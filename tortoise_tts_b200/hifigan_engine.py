@@ -1,11 +1,11 @@
-"""HiFiGAN decoder of the reference's `api_fast` path on the sm_100a kernels (SURVEY §8f row 3).
+"""HiFiGAN decoder of the reference's `api_fast` path on the sm_90a kernels (SURVEY §8f row 3).
 
 Mirrors `HifiganGenerator.inference(gpt_latents, g=speaker_latent)` (tortoise/models/hifigan_decoder.py:270-294, forward
 240-268, ResBlock1 83-97) as `api_fast.py:221-227` configures it: GPT latents [L, 1024] -> linear x 4 -> linear x 24000/22050
 -> conv_pre(k 7) + cond_layer(speaker) -> 4 x [leaky_relu 0.1 -> ConvTranspose1d (x 8, 8, 2, 2) -> mean of three ResBlock1
 (k 3 / 7 / 11, dilations 1 / 3 / 5)] -> leaky_relu (0.01) -> conv_post(k 7) -> tanh: 256 samples per input frame at 24 kHz.
 
-Everything is token-major `[T, C]` and every convolution is one tcgen05 GEMM (`ttb_gemm`, conv taps = shifted TMA loads,
+Everything is token-major `[T, C]` and every convolution is one wgmma GEMM (`ttb_gemm`, conv taps = shifted TMA loads,
 `tap_dilation` for the dilated ones):
   * operands are the error-compensated bf16 triple [hi | lo | hi] x [Wh | Wh | Wl] (fp32-grade products; a vocoder
     stacks ~45 convolutions and plain bf16 operands would not hold the 0.03 waveform tolerance), written by

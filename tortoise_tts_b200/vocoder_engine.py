@@ -1,7 +1,7 @@
-"""UnivNet vocoder on the sm_100a kernels (hot loop 3, SURVEY §8 row a13).
+"""UnivNet vocoder on the sm_90a kernels (hot loop 3, SURVEY §8 row a13).
 
 Mirrors `UnivNetGenerator.inference(c, z)` (tortoise/models/vocoder.py:300-312). Weight-norm is folded at load
-time (`remove_weight_norm`, vocoder.py:290-298). The kernel-predictor's kernel_conv + bias_conv become ONE tcgen05
+time (`remove_weight_norm`, vocoder.py:290-298). The kernel-predictor's kernel_conv + bias_conv become ONE wgmma
 GEMM whose rows are permuted so that its output is directly the per-frame kernel block the fused LVC kernel reads.
 """
 import torch
