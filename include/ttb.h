@@ -24,7 +24,8 @@ int ttb_version(void);
 int ttb_device_ok(void);
 
 /* ---------------------------------------------------------------- dense contraction (wgmma) */
-enum { TTB_ACT_NONE = 0, TTB_ACT_GELU_NEW = 1, TTB_ACT_SILU = 2, TTB_ACT_GEGLU = 3, TTB_ACT_LRELU02 = 4, TTB_ACT_TANH = 5 };
+enum { TTB_ACT_NONE = 0, TTB_ACT_GELU_NEW = 1, TTB_ACT_SILU = 2, TTB_ACT_GEGLU = 3, TTB_ACT_LRELU02 = 4, TTB_ACT_TANH = 5,
+       TTB_ACT_GELU_ERF = 6 /* exact 0.5 x (1 + erf(x / sqrt 2)): HF ACT2FN['gelu'] of the wav2vec2 aligner */ };
 
 typedef struct TtbGemmArgs {
   const void* A;        /* bf16 [batch, rows, lda] activations (K contiguous) */
@@ -316,6 +317,26 @@ int ttb_voc_lvc_gate(const float* y, int C, int L, int hop, const float* kernels
 /* channel-major fp32 [C, L] -> token-major bf16 [L, ldo] (feeds the kernel-predictor GEMM). split != 0 writes the
  * error-compensated triple [hi | lo | hi] (ldo >= 3C) to be contracted with weights packed as [Wh | Wh | Wl]. */
 int ttb_voc_to_tokens_bf16(const float* x, int C, int L, void* out, int ldo, int split, void* stream);
+
+/* ---------------------------------------------------------------- wav2vec2 CTC aligner (prompt redaction) */
+/* Wav2Vec2ForCTC forward of Wav2VecAlignment.align (utils/wav2vec_alignment.py:58-70); the projections, strided convs,
+ * grouped positional conv (TTB_ACT_GELU_ERF epilogue), encoder LayerNorms and attention run on ttb_gemm, ttb_layernorm
+ * and ttb_attention. */
+/* clip_norm = (x - mean) / sqrt(var + 1e-7) over the whole 16 kHz clip, var unbiased (wav2vec_alignment.py:65),
+ * deterministic (no atomics), fused with feature-extractor conv layer 0 (Conv1d(1, C, 10, stride 5) + bias), LayerNorm
+ * over the C channels (eps 1e-5) and exact GELU (HF Wav2Vec2LayerNormConvLayer). x fp32 [n]; w fp32 [C, 10]; b, g, beta
+ * fp32 [C]; C a multiple of 32, <= 512. stats: device scratch of 2 floats (mean, sqrt(var + 1e-7) are left there).
+ * Writes bf16 token-major [(n - 10) / 5 + 1, ldo]. */
+int ttb_wav2vec_conv0(const float* x, int n, const float* w, const float* b, const float* g, const float* beta, int C,
+                      float* stats, void* out_bf16, int ldo, void* stream);
+/* y = LN(x) * g + b (eps 1e-5), then exact GELU if gelu != 0, over fp32 rows x [M, D] (D a multiple of 128, <= 1024);
+ * writes bf16 and/or fp32 [M, D]. The LayerNorm + GELU after feature-extractor conv layers 1-6
+ * (HF Wav2Vec2LayerNormConvLayer). */
+int ttb_layernorm_act(const float* x, int M, int D, const float* g, const float* b, int gelu, void* out_bf16,
+                      float* out_f32, void* stream);
+/* out[t] = argmax_j x[t, j] over fp32 [T, V] (logits.argmax(-1), wav2vec_alignment.py:70,97): the first index on ties and
+ * NaN above every number, as torch.argmax. out int32 [T]. */
+int ttb_argmax_rows(const float* x, int T, int V, int* out, void* stream);
 
 #ifdef __cplusplus
 }

@@ -10,7 +10,7 @@ sampling / diffusion randomness comes from device generators seeded by `use_dete
 """
 import os
 import random
-from time import time
+from time import time, perf_counter
 
 import torch
 
@@ -25,6 +25,8 @@ from . import parallel
 
 DEFAULT_MODELS_DIR = os.path.join(os.path.expanduser("~"), ".cache", "tortoise", "models")
 MODELS_DIR = os.environ.get("TORTOISE_MODELS_DIR", DEFAULT_MODELS_DIR)
+# the two Hugging Face repositories Wav2VecAlignment loads (utils/wav2vec_alignment.py:53,55)
+ALIGNER_REPOS = ("jbetker/wav2vec2-large-robust-ft-libritts-voxpopuli", "jbetker/tacotron-symbols")
 MODELS = ("autoregressive.pth", "classifier.pth", "clvp2.pth", "cvvp.pth", "diffusion_decoder.pth", "vocoder.pth",
           "rlg_auto.pth", "rlg_diffuser.pth")
 
@@ -191,18 +193,45 @@ class _Tokenizer:
         return txt.replace("[SPACE]", " ").replace("[STOP]", "").replace("[UNK]", "")
 
 
+def _hf_cache_snapshot(repo):
+    """Directory of the cached snapshot of a Hugging Face repository, found on disk only (no network), or None."""
+    home = os.environ.get("HF_HOME", os.path.join(os.path.expanduser("~"), ".cache", "huggingface"))
+    for root in (os.environ.get("HF_HUB_CACHE"), os.path.join(home, "hub")):
+        if not root:
+            continue
+        d = os.path.join(root, "models--" + repo.replace("/", "--"))
+        ref = os.path.join(d, "refs", "main")
+        if os.path.exists(ref):
+            with open(ref) as f:
+                snap = os.path.join(d, "snapshots", f.read().strip())
+            if os.path.isdir(snap):
+                return snap
+        snaps = os.path.join(d, "snapshots")
+        if os.path.isdir(snaps) and os.listdir(snaps):
+            return os.path.join(snaps, sorted(os.listdir(snaps))[-1])
+    return None
+
+
 class TextToSpeech:
     def __init__(self, autoregressive_batch_size=None, models_dir=MODELS_DIR, enable_redaction=True, kv_cache=False,
                  use_deepspeed=False, half=False, device=None, tokenizer_vocab_file=None, tokenizer_basic=False,
-                 state_dicts=None, config: ModelConfig = None):
+                 state_dicts=None, config: ModelConfig = None, aligner_dir=None):
         """`state_dicts` (dict with keys autoregressive/diffusion/clvp/vocoder) bypasses models_dir (synthetic
-        checkpoints); `config` overrides the full-size ModelConfig (tests)."""
+        checkpoints); `config` overrides the full-size ModelConfig (tests).
+
+        With `enable_redaction` (the default, as in the reference) the `[bracketed]` parts of a text are cut from the
+        returned audio by a wav2vec2 CTC aligner, loaded at the first such text from: state_dicts["wav2vec"] =
+        (config, state dict, vocab) (synth.synth_wav2vec), else `aligner_dir` / TORTOISE_WAV2VEC_DIR (an HF checkpoint
+        directory; vocab.json from TORTOISE_WAV2VEC_VOCAB or that directory), else the local Hugging Face cache of
+        ALIGNER_REPOS."""
         if not torch.cuda.is_available():
             raise RuntimeError("tortoise_tts_b200 needs a CUDA device (sm_90a); there is no CPU path")
         lib.load()
         self.models_dir = models_dir
         self.autoregressive_batch_size = autoregressive_batch_size  # accepted for API parity; one batch is used
-        self.enable_redaction = False  # wav2vec redaction is out of scope (SURVEY §2 #15)
+        self.enable_redaction = bool(enable_redaction)
+        self._aligner_dir = aligner_dir
+        self.aligner = None              # loaded at the first tts() text with a '[' (load_aligner)
         self.kv_cache = kv_cache
         self.device = torch.device(device if device is not None else "cuda")
         if self.device.type == "cuda":
@@ -231,6 +260,7 @@ class TextToSpeech:
         self._rlg_sd = (state_dicts.get("rlg_auto"), state_dicts.get("rlg_diffuser"))
         self.rlg_auto = self.rlg_diffusion = None
         self._cvvp_sd = state_dicts.get("cvvp")
+        self._wav2vec = state_dicts.get("wav2vec")
         self.cvvp = None                 # the CVVP model is only loaded if used (api.py:234,252-256)
         self.last_timings = {}
         self.debug_capture = False
@@ -255,6 +285,29 @@ class TextToSpeech:
         if sd is None:
             sd = torch.load(get_model_path("cvvp.pth", self.models_dir), map_location="cpu")
         self.cvvp = CVVPEngine(sd, self.cfg, self.device)
+
+    def load_aligner(self):
+        """The wav2vec2 aligner of prompt redaction (Wav2VecAlignment, api.py:204-205); see __init__ for the sources."""
+        from .redaction import Aligner, CTCCharTokenizer
+        from .wav2vec_engine import Wav2VecEngine, load_checkpoint
+        if self._wav2vec is not None:
+            cfg, sd, vocab = self._wav2vec
+            tok = CTCCharTokenizer(vocab)
+        else:
+            mdir = self._aligner_dir or os.environ.get("TORTOISE_WAV2VEC_DIR")
+            vocab = os.environ.get("TORTOISE_WAV2VEC_VOCAB")
+            if vocab is None and mdir and os.path.exists(os.path.join(mdir, "vocab.json")):
+                vocab = mdir
+            mdir = mdir or _hf_cache_snapshot(ALIGNER_REPOS[0])
+            vocab = vocab or _hf_cache_snapshot(ALIGNER_REPOS[1])
+            if not mdir or not os.path.exists(os.path.join(mdir, "config.json")) or not vocab:
+                raise FileNotFoundError(
+                    "prompt redaction needs the wav2vec2 aligner: pass aligner_dir=... or set TORTOISE_WAV2VEC_DIR (and "
+                    "TORTOISE_WAV2VEC_VOCAB), or place %s and %s in the local Hugging Face cache; or construct "
+                    "TextToSpeech(enable_redaction=False)" % ALIGNER_REPOS)
+            cfg, sd = load_checkpoint(mdir)
+            tok = CTCCharTokenizer.from_path(vocab)
+        self.aligner = Aligner(Wav2VecEngine(cfg, sd, self.device), tok)
 
     def get_random_conditioning_latents(self):
         """≙ api.py:301-309 (rlg_auto.pth / rlg_diffuser.pth, lazily loaded)."""
@@ -426,6 +479,17 @@ class TextToSpeech:
                 e[3].record()
                 timers.append(e)
             ev[3].record()
+            t_red = None
+            if self.enable_redaction and text is not None and "[" in text:
+                # api.py:583-587: every candidate this rank rendered, before the waveforms are exchanged
+                if self.aligner is None:
+                    self.load_aligner()
+                torch.cuda.synchronize()
+                t0 = perf_counter()
+                for j in wavs:
+                    wavs[j] = self.aligner.redact(wavs[j].reshape(1, -1), text)
+                torch.cuda.synchronize()
+                t_red = (perf_counter() - t0) * 1e3
             res = []
             for j in range(best_codes.shape[0]):
                 owner = plan[j][0]
@@ -441,6 +505,8 @@ class TextToSpeech:
             self.last_timings = {"ar_ms": ev[0].elapsed_time(ev[1]), "clvp_ms": ev[1].elapsed_time(ev[2]),
                                  "latents_ms": t_lat, "diffusion_ms": t_diff, "vocoder_ms": t_voc,
                                  "device_total_ms": ev[0].elapsed_time(ev[3])}
+            if t_red is not None:
+                self.last_timings["redaction_ms"] = t_red
         out = res if len(res) > 1 else res[0]
         if return_deterministic_state:
             return out, (seed, text, voice_samples, conditioning_latents)

@@ -8,7 +8,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libttb.so")
 STAMP = LIB + ".stamp"      # content hash of the sources the library was built from (travels with the .so)
-SOURCES = ["capi.cu", "gemm.cu", "norm.cu", "attention.cu", "flash_attn.cu", "ar.cu", "ar_step.cu", "misc.cu", "vocoder.cu", "audio.cu"]
+SOURCES = ["capi.cu", "gemm.cu", "norm.cu", "attention.cu", "flash_attn.cu", "ar.cu", "ar_step.cu", "misc.cu", "vocoder.cu", "audio.cu", "wav2vec.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "--use_fast_math",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-O3"]
 

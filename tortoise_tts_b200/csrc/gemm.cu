@@ -329,6 +329,7 @@ __global__ void gemm_ref_kernel(const __nv_bfloat16* A, long long a_bstride, int
     if (ep.act == TTB_ACT_GELU_NEW) v = gelu_new(v);
     else if (ep.act == TTB_ACT_SILU) v = silu(v);
     else if (ep.act == TTB_ACT_LRELU02) v = leaky(v, 0.2f);
+    else if (ep.act == TTB_ACT_GELU_ERF) v = gelu_erf(v);
     if (ep.residual) v += ep.residual[(long long)bz * ep.res_bstride + (long long)m * ep.ldr + n];
   }
   if (ep.out_f32) ep.out_f32[(long long)bz * ep.outf_bstride + (long long)m * ep.ldo + on] = v;

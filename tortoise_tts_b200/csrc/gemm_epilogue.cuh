@@ -39,6 +39,7 @@ TTB_DEVINL float epi_act(float x) {
   if (ACT == TTB_ACT_SILU) return silu(x);
   if (ACT == TTB_ACT_LRELU02) return leaky(x, 0.2f);
   if (ACT == TTB_ACT_TANH) return tanhf(x);
+  if (ACT == TTB_ACT_GELU_ERF) return gelu_erf(x);
   return x;
 }
 
@@ -209,6 +210,7 @@ TTB_DEVINL void gemm_epilogue_dispatch(uint32_t blk, int n0, int N, int m_base, 
     case TTB_ACT_SILU: gemm_epilogue_tile<BN, TTB_ACT_SILU>(blk, n0, N, m_base, M, lane, bz, ep, ch_begin, ch_step); break;
     case TTB_ACT_LRELU02: gemm_epilogue_tile<BN, TTB_ACT_LRELU02>(blk, n0, N, m_base, M, lane, bz, ep, ch_begin, ch_step); break;
     case TTB_ACT_TANH: gemm_epilogue_tile<BN, TTB_ACT_TANH>(blk, n0, N, m_base, M, lane, bz, ep, ch_begin, ch_step); break;
+    case TTB_ACT_GELU_ERF: gemm_epilogue_tile<BN, TTB_ACT_GELU_ERF>(blk, n0, N, m_base, M, lane, bz, ep, ch_begin, ch_step); break;
     default: gemm_epilogue_tile<BN, TTB_ACT_NONE>(blk, n0, N, m_base, M, lane, bz, ep, ch_begin, ch_step); break;
   }
 }

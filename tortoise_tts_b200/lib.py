@@ -11,6 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libttb.so")
 
 ACT_NONE, ACT_GELU_NEW, ACT_SILU, ACT_GEGLU, ACT_LRELU02, ACT_TANH = 0, 1, 2, 3, 4, 5
+ACT_GELU_ERF = 6
 
 
 class TtbError(RuntimeError):
@@ -77,6 +78,7 @@ SYMBOLS = [
     "ttb_ar_step_workspace", "ttb_ar_step_setup", "ttb_ar_decode_step", "ttb_ar_step_store_prefix",
     "ttb_audio_resample", "ttb_audio_stft_mel", "ttb_mean_rows", "ttb_equal_linear",
     "ttb_pair_exchange", "ttb_enable_peer_access", "ttb_peer_alloc", "ttb_peer_open", "ttb_peer_close", "ttb_peer_free",
+    "ttb_wav2vec_conv0", "ttb_layernorm_act", "ttb_argmax_rows",
 ]
 
 
@@ -435,3 +437,19 @@ def voc_lvc_gate(y, Cc, L, hop, kernels, ldk, koff, bias, ldb, boff, x):
 def voc_to_tokens_bf16(x, Cc, L, out, ldo, split=False):
     _chk(load().ttb_voc_to_tokens_bf16(_p(_f32(x)), Cc, L, _p(_bf(out)), ldo, 1 if split else 0, _stream()),
          "ttb_voc_to_tokens_bf16")
+
+
+def wav2vec_conv0(x, n, w, b, g, beta, Cc, stats, out, ldo):
+    """Clip normalisation + wav2vec2 feature-extractor conv layer 0 + LayerNorm + GELU (include/ttb.h)."""
+    _chk(load().ttb_wav2vec_conv0(_p(_f32(x)), n, _p(_f32(w)), _p(_f32(b)), _p(_f32(g)), _p(_f32(beta)), Cc,
+                                  _p(_f32(stats)), _p(_bf(out)), ldo, _stream()), "ttb_wav2vec_conv0")
+
+
+def layernorm_act(x, M, D, g, b, gelu=False, out_bf16=None, out_f32=None):
+    _chk(load().ttb_layernorm_act(_p(_f32(x)), M, D, _p(_f32(g)), _p(_f32(b)), 1 if gelu else 0, _p(_bf(out_bf16)),
+                                  _p(_f32(out_f32)), _stream()), "ttb_layernorm_act")
+
+
+def argmax_rows(x, T, V, out):
+    assert out.dtype == torch.int32, out.dtype
+    _chk(load().ttb_argmax_rows(_p(_f32(x)), T, V, _p(out), _stream()), "ttb_argmax_rows")

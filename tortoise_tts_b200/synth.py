@@ -304,6 +304,73 @@ def synth_rlg(C, seed=0):
     return sd
 
 
+W2V_VOCAB = ["<pad>", "<s>", "</s>", "<unk>", "|"] + list("'abcdefghijklmnopqrstuvwxyz,.!?-")
+
+
+def wav2vec_config(size="full"):
+    """HF Wav2Vec2Config fields of the redaction aligner: "full" = wav2vec2-large-robust (24 x 1024, 16 heads, FF 4096),
+    "small" = the same architecture at 2 x 256 (tests)."""
+    full = size == "full"
+    H = 1024 if full else 256
+    return {
+        "model_type": "wav2vec2", "architectures": ["Wav2Vec2ForCTC"],
+        "do_stable_layer_norm": True, "feat_extract_norm": "layer", "conv_bias": True,
+        "feat_extract_activation": "gelu", "hidden_act": "gelu",
+        "conv_dim": [512 if full else 256] * 7, "conv_kernel": [10, 3, 3, 3, 3, 2, 2], "conv_stride": [5, 2, 2, 2, 2, 2, 2],
+        "hidden_size": H, "num_attention_heads": H // 64, "intermediate_size": 4 * H,
+        "num_hidden_layers": 24 if full else 2,
+        "num_conv_pos_embeddings": 128 if full else 32, "num_conv_pos_embedding_groups": 16 if full else 4,
+        "layer_norm_eps": 1e-5, "vocab_size": len(W2V_VOCAB), "pad_token_id": 0,
+        "hidden_dropout": 0.0, "attention_dropout": 0.0, "activation_dropout": 0.0, "feat_proj_dropout": 0.0,
+        "final_dropout": 0.0, "layerdrop": 0.0, "mask_time_prob": 0.0,
+    }
+
+
+def synth_wav2vec(cfg="small", seed=0):
+    """Seeded Wav2Vec2ForCTC checkpoint for the redaction aligner: (config dict, state dict in the HF key layout,
+    character vocab {token: id}). `cfg`: "small", "full" or a config dict (wav2vec_config). The positional conv's weight
+    norm is stored in the `parametrizations.weight.original0/1` form. Not part of synth_all."""
+    if isinstance(cfg, str):
+        cfg = wav2vec_config(cfg)
+    g = _Gen(seed * 1000 + 9)
+    C, H, FF = cfg["conv_dim"][0], cfg["hidden_size"], cfg["intermediate_size"]
+    V, k, G = cfg["vocab_size"], cfg["num_conv_pos_embeddings"], cfg["num_conv_pos_embedding_groups"]
+    sd = {}
+    p = "wav2vec2."
+    cin = 1
+    for i, kk in enumerate(cfg["conv_kernel"]):
+        q = p + f"feature_extractor.conv_layers.{i}."
+        sd[q + "conv.weight"] = g.lin((C, cin, kk), cin * kk)
+        sd[q + "conv.bias"] = g.bias(C)
+        sd[q + "layer_norm.weight"] = g.gamma(C)
+        sd[q + "layer_norm.bias"] = g.beta(C)
+        cin = C
+    q = p + "feature_projection."
+    sd[q + "layer_norm.weight"], sd[q + "layer_norm.bias"] = g.gamma(C), g.beta(C)
+    sd[q + "projection.weight"], sd[q + "projection.bias"] = g.lin((H, C), C), g.bias(H)
+    q = p + "encoder.pos_conv_embed.conv."
+    v = g.lin((H, H // G, k), k * H // G, 0.5)
+    norm = v.permute(2, 0, 1).reshape(k, -1).norm(dim=1).reshape(1, 1, k)
+    sd[q + "bias"] = g.bias(H)
+    sd[q + "parametrizations.weight.original0"] = norm * (1.0 + g.normal(norm.shape, 0.05))
+    sd[q + "parametrizations.weight.original1"] = v
+    sd[p + "encoder.layer_norm.weight"], sd[p + "encoder.layer_norm.bias"] = g.gamma(H), g.beta(H)
+    for l in range(cfg["num_hidden_layers"]):
+        q = p + f"encoder.layers.{l}."
+        for n in ("q", "k", "v", "out"):
+            sd[q + f"attention.{n}_proj.weight"] = g.lin((H, H), H)
+            sd[q + f"attention.{n}_proj.bias"] = g.bias(H)
+        sd[q + "layer_norm.weight"], sd[q + "layer_norm.bias"] = g.gamma(H), g.beta(H)
+        sd[q + "final_layer_norm.weight"], sd[q + "final_layer_norm.bias"] = g.gamma(H), g.beta(H)
+        sd[q + "feed_forward.intermediate_dense.weight"] = g.lin((FF, H), H)
+        sd[q + "feed_forward.intermediate_dense.bias"] = g.bias(FF)
+        sd[q + "feed_forward.output_dense.weight"] = g.lin((H, FF), FF, 0.5)
+        sd[q + "feed_forward.output_dense.bias"] = g.bias(H)
+    sd["lm_head.weight"], sd["lm_head.bias"] = g.lin((V, H), H, 2.0), g.bias(V, 0.5)
+    vocab = {t: i for i, t in enumerate(W2V_VOCAB[:V])}
+    return cfg, sd, vocab
+
+
 def synth_all(cfg: ModelConfig, seed=0, suppress_stop=True):
     return {
         "autoregressive": synth_autoregressive(cfg, seed, suppress_stop),
