@@ -161,6 +161,14 @@ int ttb_ar_store_prefix(const void* qkv, int P, int H, void* prefix_k, void* pre
 int ttb_ar_sample(const float* logits, int ld_logits, int V, int B, const float* uniforms, int ld_u, uint32_t* seen,
                   int* codes, int ld_codes, int* finished, TtbArState* state, float temperature, int top_k, float top_p,
                   float rep_penalty, int stop_token, int advance, void* stream);
+/* ttb_ar_sample with the reference's TypicalLogitsWarper(mass=typical_mass) (utils/typical_sampling.py:11-33) between
+ * the repetition penalty and the temperature: only the typical set T of the penalised scores can be drawn (top-k keeps
+ * min(top_k, |T|) tokens). typical_mass in (0, 1], else -1. Where the cumulative mass never reaches typical_mass
+ * (mass 1 under rounding) every token is kept; the reference raises an IndexError there. */
+int ttb_ar_sample_typical(const float* logits, int ld_logits, int V, int B, const float* uniforms, int ld_u,
+                          uint32_t* seen, int* codes, int ld_codes, int* finished, TtbArState* state, float temperature,
+                          int top_k, float top_p, float rep_penalty, int stop_token, int advance, float typical_mass,
+                          void* stream);
 /* fix_autoregressive_output (api.py:87-114) for every row + calm-token trim length (api.py:547-556) */
 int ttb_ar_fix_codes(int* codes, int B, int L, int stop_token, int* trim_len, void* stream);
 /* rows of an embedding table + optional positional table -> fp32 [n, D]; ids int32, pos int32 (or NULL) */

@@ -147,6 +147,18 @@ def do_spectrogram_diffusion(diffusion_model, diffuser, latents, conditioning_la
     return mel.unsqueeze(0)
 
 
+def _typical_mass(typical_sampling, typical_mass):
+    """The engine's typical_mass for the tts() kwargs `typical_sampling` / `typical_mass`: None when the filter is off.
+    A mass outside (0, 1] raises ValueError. The reference raises an IndexError where the cumulative mass never reaches
+    typical_mass (mass 1 under rounding); here every token is kept instead."""
+    if not typical_sampling:
+        return None
+    m = float(typical_mass)
+    if not 0.0 < m <= 1.0:
+        raise ValueError("typical_mass must lie in (0, 1], got %r" % (typical_mass,))
+    return m
+
+
 def classify_audio_clip(clip):
     """api.py:133-145 (AudioMiniEncoderWithClassifierHead): not on the synthesis path; out of scope (SURVEY §8f-4)."""
     raise NotImplementedError("classify_audio_clip is outside the hot path this engine replaces (SURVEY §8f-4)")
@@ -383,10 +395,14 @@ class TextToSpeech:
     def tts(self, text, voice_samples=None, conditioning_latents=None, k=1, verbose=True, use_deterministic_seed=None,
             return_deterministic_state=False, num_autoregressive_samples=512, temperature=.8, length_penalty=1,
             repetition_penalty=2.0, top_p=.8, max_mel_tokens=500, cvvp_amount=.0, diffusion_iterations=100,
-            cond_free=True, cond_free_k=2, diffusion_temperature=1.0, text_tokens=None, top_k=50, **hf_generate_kwargs):
-        """≙ TextToSpeech.tts (api.py:334-597). `text_tokens` (list of BPE ids) may be given instead of `text`."""
+            cond_free=True, cond_free_k=2, diffusion_temperature=1.0, text_tokens=None, top_k=50, typical_sampling=False,
+            typical_mass=.9, **hf_generate_kwargs):
+        """≙ TextToSpeech.tts (api.py:334-597). `text_tokens` (list of BPE ids) may be given instead of `text`.
+        `typical_sampling` / `typical_mass` are the reference's generate kwargs of the same names (api.py:361-364): the
+        sampler keeps only the typical set of mass `typical_mass` (in (0, 1]) of the penalised scores."""
         if hf_generate_kwargs:
             raise TypeError(f"unsupported generate kwargs: {sorted(hf_generate_kwargs)}")
+        typical = _typical_mass(typical_sampling, typical_mass)
         seed = self.deterministic_state(seed=use_deterministic_seed)
         # api.py:395-401 (after the seeding, so that the random crop / random voice follow use_deterministic_seed)
         auto_conds = None                 # the conditioning MELs: only known when the clips themselves are given
@@ -418,7 +434,8 @@ class TextToSpeech:
             codes = self.autoregressive.generate(auto_cond, toks, hi - lo, max_mel_tokens, uniforms=uniforms,
                                                  temperature=temperature, top_k=top_k, top_p=top_p,
                                                  repetition_penalty=repetition_penalty,
-                                                 pos_mode="ref_kv_quirk" if self.kv_cache else "train_consistent")
+                                                 pos_mode="ref_kv_quirk" if self.kv_cache else "train_consistent",
+                                                 typical_mass=typical)
             nb, L = codes.shape
             trim = torch.empty(nb, dtype=torch.int32, device=dev)
             lib.ar_fix_codes(codes, nb, L, self.cfg.stop_mel_token, trim)

@@ -24,7 +24,7 @@ from .conditioning_engine import ConditioningEngine, RandomLatentEngine
 from .hifigan_engine import HifiganEngine
 from . import lib
 from . import parallel
-from .api import MODELS_DIR, _Tokenizer, _default_mel_norms
+from .api import MODELS_DIR, _Tokenizer, _default_mel_norms, _typical_mass
 # module-level names callers of tortoise/api_fast.py import from it (api_fast.py:52-171)
 from .api import pad_or_truncate, format_conditioning, pick_best_batch_size_for_gpu, classify_audio_clip  # noqa: F401
 
@@ -209,13 +209,16 @@ class TextToSpeech:
 
     def tts(self, text, voice_samples=None, k=1, verbose=True, use_deterministic_seed=None,
             num_autoregressive_samples=512, temperature=.8, length_penalty=1, repetition_penalty=2.0, top_p=.8,
-            max_mel_tokens=500, cvvp_amount=.0, text_tokens=None, top_k=50, **hf_generate_kwargs):
+            max_mel_tokens=500, cvvp_amount=.0, text_tokens=None, top_k=50, typical_sampling=False, typical_mass=.9,
+            **hf_generate_kwargs):
         """≙ api_fast.py:421-507: ONE sampled sequence (`num_return_sequences=1`; the generation limit is the model's
         `max_mel_tokens - 1`, the `max_mel_tokens` argument is not used by the reference either) -> latents of
         `UnifiedVoice.forward(return_latent=True)` over the raw codes (stop token included, no `fix_autoregressive_output`)
-        -> HiFiGAN. Returns fp32 [1, 1, samples] on the device."""
+        -> HiFiGAN. Returns fp32 [1, 1, samples] on the device. `typical_sampling` / `typical_mass`: as in api.tts
+        (api_fast.py:484-495 passes them to the generator the same way)."""
         if hf_generate_kwargs:
             raise TypeError(f"unsupported generate kwargs: {sorted(hf_generate_kwargs)}")
+        typical = _typical_mass(typical_sampling, typical_mass)
         seed, toks, auto = self._inputs(text, voice_samples, text_tokens, use_deterministic_seed)
         if verbose:
             print("Generating autoregressive samples..")
@@ -230,7 +233,8 @@ class TextToSpeech:
             uniforms = torch.rand(1, n_max, generator=g, device=self.device)
             codes = self.autoregressive.generate(auto, toks, 1, n_max, uniforms=uniforms, temperature=temperature,
                                                  top_k=top_k, top_p=top_p, repetition_penalty=repetition_penalty,
-                                                 pos_mode=self._pos_mode(), use_graph=self.device.type == "cuda")
+                                                 pos_mode=self._pos_mode(), use_graph=self.device.type == "cuda",
+                                                 typical_mass=typical)
             hit = (codes[0] == self.cfg.stop_mel_token).nonzero()
             n = int(hit[0].item()) + 1 if hit.numel() > 0 else n_max          # HF returns the stop token it sampled
             mark(1)

@@ -242,9 +242,7 @@ class AREngine:
         x, ws = st["x"], st["ws"]
         if st["mode"] == "fused":
             self._step_handle(st, sp["pos_mode"]).step()
-            lib.ar_sample(st["logits"], self.V, self.V, B, st["uniforms"], Nmax, st["seen"], st["codes"], Nmax,
-                          st["finished"], st["state"], sp["temperature"], sp["top_k"], sp["top_p"], sp["rep_penalty"],
-                          self.cfg.stop_mel_token, advance=True)
+            self._sample(sp, st["logits"], self.V, st)
             return
         hd = self._step_handle(st, sp["pos_mode"]) if st["mode"] == "mixed" else None
         lib.ar_embed_step(st["codes"], Nmax, st["state"], self.w.mel_emb, self.w.mel_pos, B, D, sp["pos_mode"], x)
@@ -284,9 +282,18 @@ class AREngine:
         lib.residual_layernorm(x, B, D, prev[0], prev[1], B * D, prev[2], self.w.lnf_g, self.w.lnf_b, self.w.fn_g,
                                self.w.fn_b, out_bf16=st["hn"])
         lib.gemm(st["hn"], self.w.w_head, M=B, N=self.V, K=D, bias=self.w.b_head, out_f32=st["logits"], w_static=ws_ln)
-        lib.ar_sample(st["logits"], self.V, self.V, B, st["uniforms"], Nmax, st["seen"], st["codes"], Nmax,
-                      st["finished"], st["state"], sp["temperature"], sp["top_k"], sp["top_p"], sp["rep_penalty"],
-                      self.cfg.stop_mel_token, advance=True)
+        self._sample(sp, st["logits"], self.V, st)
+
+    def _sample(self, sp, logits, ld_logits, ch):
+        """The sampler over the logits of one chain (ld_logits = 0: row 0 for every candidate); the typical-set entry
+        when `sp` turns the filter on."""
+        Nmax = ch["Nmax"]
+        args = (logits, ld_logits, self.V, ch["B"], ch["uniforms"], Nmax, ch["seen"], ch["codes"], Nmax, ch["finished"],
+                ch["state"], sp["temperature"], sp["top_k"], sp["top_p"], sp["rep_penalty"], self.cfg.stop_mel_token)
+        if sp.get("typical_mass") is None:
+            lib.ar_sample(*args, advance=True)
+        else:
+            lib.ar_sample_typical(*args, sp["typical_mass"], advance=True)
 
     def _begin(self, cond_latent, text_tokens, B, Nmax, uniforms, seed, sp, trace_logits=None):
         """Workspace reset + prompt prefill + the first sampled token of every candidate."""
@@ -311,9 +318,7 @@ class AREngine:
             # HF's repetition penalty sees the fake prompt ids {1, start_mel} (autoregressive.py:546-548)
             ch["seen"][:, 0] = 2
             ch["seen"][:, w] |= (1 << bit) if bit < 31 else -(1 << 31)
-            lib.ar_sample(st["logits"], 0, self.V, ch["B"], ch["uniforms"], Nmax, ch["seen"], ch["codes"], Nmax,
-                          ch["finished"], ch["state"], sp["temperature"], sp["top_k"], sp["top_p"], sp["rep_penalty"],
-                          cfg.stop_mel_token, advance=True)
+            self._sample(sp, st["logits"], 0, ch)
         return st
 
     _SNAP = ("state", "codes", "seen", "finished")
@@ -361,18 +366,28 @@ class AREngine:
         return cs[0].clone() if len(cs) == 1 else torch.cat(cs, dim=0)
 
     @staticmethod
-    def _sampling(temperature, top_k, top_p, repetition_penalty, pos_mode):
-        return dict(temperature=float(temperature), top_k=int(top_k), top_p=float(top_p),
-                    rep_penalty=float(repetition_penalty), pos_mode=1 if pos_mode == "ref_kv_quirk" else 0)
+    def _sampling(temperature, top_k, top_p, repetition_penalty, pos_mode, typical_mass=None):
+        """The sampling parameters of a decode; also the key of the captured step graph, so a change of any of them
+        (the typical mass included) captures a new graph. typical_mass None = no typical filter."""
+        sp = dict(temperature=float(temperature), top_k=int(top_k), top_p=float(top_p),
+                  rep_penalty=float(repetition_penalty), pos_mode=1 if pos_mode == "ref_kv_quirk" else 0)
+        if typical_mass is not None:
+            m = float(typical_mass)
+            if not 0.0 < m <= 1.0:
+                raise ValueError("typical_mass must lie in (0, 1], got %r" % (typical_mass,))
+            sp["typical_mass"] = m
+        return sp
 
     def generate(self, cond_latent, text_tokens, num_candidates, max_new, uniforms=None, seed=None, temperature=0.8,
                  top_k=50, top_p=0.8, repetition_penalty=2.0, pos_mode="ref_kv_quirk", use_graph=True,
-                 stop_check_every=32, trace_logits=None):
+                 stop_check_every=32, trace_logits=None, typical_mass=None):
         """≙ num_candidates/bs calls of UnifiedVoice.inference_speech (autoregressive.py:535-563), all candidates in
         ONE batch with a shared-prefix KV cache. Returns int32 codes [num_candidates, max_new] padded with the
-        stop token (api.py:425-426). `uniforms` [B, max_new] injects the sampling randomness (parity mode)."""
+        stop token (api.py:425-426). `uniforms` [B, max_new] injects the sampling randomness (parity mode).
+        `typical_mass` (in (0, 1]) turns on the reference's typical-set filter (TypicalLogitsWarper after the repetition
+        penalty, autoregressive.py:558); None leaves it off."""
         B, Nmax = int(num_candidates), int(max_new)
-        sp = self._sampling(temperature, top_k, top_p, repetition_penalty, pos_mode)
+        sp = self._sampling(temperature, top_k, top_p, repetition_penalty, pos_mode, typical_mass)
         if trace_logits is not None:
             use_graph = False
         st = self._begin(cond_latent, text_tokens, B, Nmax, uniforms, seed, sp, trace_logits)
@@ -400,14 +415,14 @@ class AREngine:
 
     def generate_stream(self, cond_latent, text_tokens, max_new, first_block, block, uniforms=None, seed=None,
                         temperature=0.8, top_k=50, top_p=0.8, repetition_penalty=2.0, pos_mode="ref_kv_quirk",
-                        use_graph=True):
+                        use_graph=True, typical_mass=None):
         """ONE sequence decoded block-wise: ≙ the token stream of `GPT2InferenceModel.generate_stream` /
         `sample_stream` (autoregressive.py:565-574, stream_generator.py:916-1000), which yields every sampled token
         INCLUDING the stop token and ends after it (or after `max_new` tokens). A generator of `(codes, ended)`:
         `codes` = int32 [n] all tokens so far, after the first `first_block` tokens, then every `block` tokens, and a
         last time when the stream has ended (`ended` True; the stop token, if any, is the last element)."""
         Nmax = int(max_new)
-        sp = self._sampling(temperature, top_k, top_p, repetition_penalty, pos_mode)
+        sp = self._sampling(temperature, top_k, top_p, repetition_penalty, pos_mode, typical_mass)
         st = self._begin(cond_latent, text_tokens, 1, Nmax, uniforms, seed, sp)
         if use_graph and Nmax > 1:
             self._ensure_graph(st, sp)

@@ -29,7 +29,8 @@ __global__ void ar_embed_step_kernel(const int* __restrict__ codes, int ld_codes
 // ------------------------------------------------------------------ fused sampler
 // One block (256 threads) per candidate. Radix-select of the top_k-th largest value (4 passes of 8 bits over the
 // order-preserving uint32 image of the float), gather of the survivors (<= CAP), bitonic sort by one warp,
-// softmax, top-p cut on the exclusive prefix mass, inverse-CDF draw.
+// softmax, top-p cut on the exclusive prefix mass, inverse-CDF draw. The TYPICAL instantiation first restricts the
+// row to the typical set (typical_filter below), between the repetition penalty and the temperature.
 constexpr int SAMP_THREADS = 256;
 constexpr int SAMP_CAP = 64;
 
@@ -38,11 +39,97 @@ TTB_DEVINL uint32_t f2key(float f) {
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 
+// ---- typical-set filter (TypicalLogitsWarper, reference tortoise/utils/typical_sampling.py:11-33), on the penalised
+// scores s before temperature: logp = log_softmax(s), H = -nansum(p logp), key_i = |-logp_i - H|; kept set
+// T = {i : key_i <= v}, v = the smallest key with sum_{key_j <= v} p_j >= mass (ties at v all kept, never empty).
+// key_i and p_i are recomputed from sval wherever they are needed instead of being stored: a second V-float array
+// would take the dynamic shared memory past 48 KB (opt-in attribute) and halve the blocks per SM, while recomputing is
+// a few instructions per element and pass. The recomputation uses the same rounded operations everywhere (__fsub_rn /
+// __fadd_rn cannot be contracted), so every pass sees bit-identical keys and masses.
+constexpr double TYP_QSCALE = 1099511627776.0;   // 2^40: p in [0, 1] as 64-bit fixed point (bin sums cannot overflow)
+
+TTB_DEVINL float typ_logp(float s, float m, float lz) { return __fsub_rn(__fsub_rn(s, m), lz); }  // (s - max) - logZ
+TTB_DEVINL uint32_t typ_key(float lp, float H) { return f2key(fabsf(__fadd_rn(lp, H))); }       // |-logp - H|
+TTB_DEVINL unsigned long long typ_q(float lp) { return __float2ull_rn(__fmul_rn(expf(lp), (float)TYP_QSCALE)); }
+
+// Leaves sval[i] = s_i / temperature for i in T and -inf elsewhere; returns |T| (>= 1). hist: 256 u64 of shared memory,
+// red: 32 floats. The bin masses are sums of integers, so the result does not depend on the order of the atomics.
+TTB_DEVINL int typical_filter(float* sval, int V, float temperature, float mass, unsigned long long* hist, float* red,
+                              uint32_t* s_prefix, unsigned long long* s_rem, int* s_count) {
+  float m = -INFINITY;
+  for (int i = threadIdx.x; i < V; i += SAMP_THREADS) m = fmaxf(m, sval[i]);
+  m = block_max(m, red);
+  float z = 0.f;
+  for (int i = threadIdx.x; i < V; i += SAMP_THREADS) z += expf(sval[i] - m);
+  const float lz = logf(block_sum(z, red));
+  float h = 0.f;
+  for (int i = threadIdx.x; i < V; i += SAMP_THREADS) {
+    const float lp = typ_logp(sval[i], m, lz);
+    const float t = expf(lp) * lp;
+    if (!isnan(t)) h += t;                  // nansum
+  }
+  const float H = -block_sum(h, red);
+  if (threadIdx.x == 0) { *s_prefix = 0; *s_count = 0; }
+  // radix select over the keys in ASCENDING order, weighted by mass: 4 passes of 8 bits; in each, the bin where the
+  // cumulative mass of the keys below it (within the current prefix) first reaches the remaining target
+  for (int pass = 0; pass < 4; ++pass) {
+    const int shift = 24 - 8 * pass;
+    hist[threadIdx.x] = 0ull;
+    __syncthreads();
+    const uint32_t prefix = *s_prefix;
+    const uint32_t mask = (pass == 0) ? 0u : (0xFFFFFFFFu << (shift + 8));
+    for (int base = 0; base < V; base += SAMP_THREADS) {          // uniform trip count: every lane takes part
+      const int i = base + threadIdx.x;
+      int bin = 256;
+      unsigned long long q = 0ull;
+      if (i < V) {
+        const float lp = typ_logp(sval[i], m, lz);
+        const uint32_t k = typ_key(lp, H);
+        if ((k & mask) == prefix) { bin = (int)((k >> shift) & 255u); q = typ_q(lp); }
+      }
+      if (bin < 256) atomicAdd(&hist[bin], q);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      // bins in ascending key order: the first whose cumulative mass reaches the remaining target
+      unsigned long long r = *s_rem;
+      if (pass == 0) {
+        unsigned long long total = 0ull;
+        for (int d = 0; d < 256; ++d) total += hist[d];
+        // sum_{key <= v} p >= mass, measured against the total so that mass = 1 keeps everything
+        r = (unsigned long long)ceil((double)mass * (double)total);
+        r = max(1ull, min(r, total));
+      }
+      int d = 0;
+      for (; d < 255; ++d) {
+        const unsigned long long hd = hist[d];
+        if (hd >= r) break;
+        r -= hd;
+      }
+      *s_prefix = prefix | ((uint32_t)d << shift);
+      *s_rem = r;
+    }
+    __syncthreads();
+  }
+  const uint32_t v = *s_prefix;
+  int n = 0;
+  for (int i = threadIdx.x; i < V; i += SAMP_THREADS) {
+    const float s = sval[i];
+    const bool in = typ_key(typ_logp(s, m, lz), H) <= v;
+    sval[i] = in ? s / temperature : -INFINITY;
+    n += in ? 1 : 0;
+  }
+  atomicAdd(s_count, n);
+  __syncthreads();
+  return *s_count;
+}
+
+template <bool TYPICAL>
 __global__ void __launch_bounds__(SAMP_THREADS)
 ar_sample_kernel(const float* __restrict__ logits, int ld_logits, int V, const float* __restrict__ uniforms, int ld_u,
                  uint32_t* __restrict__ seen, int* __restrict__ codes, int ld_codes, int* __restrict__ finished,
                  TtbArState* __restrict__ state, float temperature, int top_k, float top_p, float rep_penalty,
-                 int stop_token, int advance) {
+                 int stop_token, int advance, float typical_mass) {
   extern __shared__ float sval[];           // V floats: processed scores
   __shared__ int hist[256];
   __shared__ uint32_t s_prefix;
@@ -64,9 +151,20 @@ ar_sample_kernel(const float* __restrict__ logits, int ld_logits, int V, const f
   for (int i = threadIdx.x; i < V; i += SAMP_THREADS) {
     float s = lrow[i];
     if ((myseen[i >> 5] >> (i & 31)) & 1u) s = (s < 0.f) ? s * rep_penalty : s / rep_penalty;
-    sval[i] = s / temperature;
+    sval[i] = TYPICAL ? s : s / temperature;  // the typical filter sees the scores before temperature, then divides
   }
-  if (threadIdx.x == 0) { s_prefix = 0; s_remaining = min(top_k, V); s_ncand = 0; }
+  int kk = min(top_k, V);                   // top-k over the candidates: the whole row, or T with the typical filter
+  if constexpr (TYPICAL) {
+    __shared__ unsigned long long t_hist[256];
+    __shared__ unsigned long long t_rem;
+    __shared__ float t_red[32];
+    __shared__ int t_count;
+    __syncthreads();
+    // masked tokens are -inf, the lowest keys of all: with k <= |T| the select, the tie fill and every fallback of the
+    // draw only ever see tokens of T
+    kk = min(kk, typical_filter(sval, V, temperature, typical_mass, t_hist, t_red, &s_prefix, &t_rem, &t_count));
+  }
+  if (threadIdx.x == 0) { s_prefix = 0; s_remaining = kk; s_ncand = 0; }
   __syncthreads();
   // radix select: find key T of the k-th largest element. The histogram updates are aggregated per warp (the keys of a
   // logit row share their exponent byte: unaggregated, pass 0 is ~8000 atomics on two or three shared-memory words), and
@@ -121,7 +219,7 @@ ar_sample_kernel(const float* __restrict__ logits, int ld_logits, int V, const f
     __syncthreads();
   }
   const uint32_t thr = s_prefix;  // key of the k-th largest; HF keeps everything >= it (ties included)
-  const int n_ge = (min(top_k, V) - s_remaining) + s_eq;     // elements with key >= thr
+  const int n_ge = (kk - s_remaining) + s_eq;              // elements with key >= thr
   if (n_ge <= SAMP_CAP) {
     // the common case: everything that is kept fits; slot order is irrelevant (sorted below by value, then index)
     for (int i = threadIdx.x; i < V; i += SAMP_THREADS) {
@@ -283,18 +381,42 @@ extern "C" int ttb_ar_embed_step(const int* codes, int ld_codes, const TtbArStat
   return 0;
 }
 
+template <bool TYPICAL>
+static int launch_ar_sample(const char* name, const float* logits, int ld_logits, int V, int B, const float* uniforms,
+                            int ld_u, uint32_t* seen, int* codes, int ld_codes, int* finished, TtbArState* state,
+                            float temperature, int top_k, float top_p, float rep_penalty, int stop_token, int advance,
+                            float typical_mass, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (top_k <= 0 || top_k > 50) { set_error("%s: top_k=%d unsupported (1..50)", name, top_k); return -1; }
+  const size_t smem = (size_t)V * sizeof(float);
+  if (smem > 40 * 1024) { set_error("%s: vocabulary %d too large", name, V); return -1; }
+  ar_sample_kernel<TYPICAL><<<B, SAMP_THREADS, smem, st>>>(logits, ld_logits, V, uniforms, ld_u, seen, codes, ld_codes,
+                                                           finished, state, temperature, top_k, top_p, rep_penalty,
+                                                           stop_token, advance ? 1 : 0, typical_mass);
+  TTB_CHECK_LAUNCH("ar_sample_kernel");
+  return 0;
+}
+
 extern "C" int ttb_ar_sample(const float* logits, int ld_logits, int V, int B, const float* uniforms, int ld_u,
                              uint32_t* seen, int* codes, int ld_codes, int* finished, TtbArState* state,
                              float temperature, int top_k, float top_p, float rep_penalty, int stop_token, int advance,
                              void* stream) {
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (top_k <= 0 || top_k > 50) { set_error("ttb_ar_sample: top_k=%d unsupported (1..50)", top_k); return -1; }
-  const size_t smem = (size_t)V * sizeof(float);
-  if (smem > 40 * 1024) { set_error("ttb_ar_sample: vocabulary %d too large", V); return -1; }
-  ar_sample_kernel<<<B, SAMP_THREADS, smem, st>>>(logits, ld_logits, V, uniforms, ld_u, seen, codes, ld_codes, finished,
-                                                  state, temperature, top_k, top_p, rep_penalty, stop_token, advance ? 1 : 0);
-  TTB_CHECK_LAUNCH("ar_sample_kernel");
-  return 0;
+  return launch_ar_sample<false>("ttb_ar_sample", logits, ld_logits, V, B, uniforms, ld_u, seen, codes, ld_codes,
+                                 finished, state, temperature, top_k, top_p, rep_penalty, stop_token, advance, 1.f,
+                                 stream);
+}
+
+extern "C" int ttb_ar_sample_typical(const float* logits, int ld_logits, int V, int B, const float* uniforms, int ld_u,
+                                     uint32_t* seen, int* codes, int ld_codes, int* finished, TtbArState* state,
+                                     float temperature, int top_k, float top_p, float rep_penalty, int stop_token,
+                                     int advance, float typical_mass, void* stream) {
+  if (!(typical_mass > 0.f && typical_mass <= 1.f)) {
+    set_error("ttb_ar_sample_typical: typical_mass=%g outside (0, 1]", (double)typical_mass);
+    return -1;
+  }
+  return launch_ar_sample<true>("ttb_ar_sample_typical", logits, ld_logits, V, B, uniforms, ld_u, seen, codes, ld_codes,
+                                finished, state, temperature, top_k, top_p, rep_penalty, stop_token, advance,
+                                typical_mass, stream);
 }
 
 extern "C" int ttb_ar_fix_codes(int* codes, int B, int L, int stop_token, int* trim_len, void* stream) {

@@ -78,7 +78,7 @@ SYMBOLS = [
     "ttb_ar_step_workspace", "ttb_ar_step_setup", "ttb_ar_decode_step", "ttb_ar_step_store_prefix",
     "ttb_audio_resample", "ttb_audio_stft_mel", "ttb_mean_rows", "ttb_equal_linear",
     "ttb_pair_exchange", "ttb_enable_peer_access", "ttb_peer_alloc", "ttb_peer_open", "ttb_peer_close", "ttb_peer_free",
-    "ttb_wav2vec_conv0", "ttb_layernorm_act", "ttb_argmax_rows",
+    "ttb_wav2vec_conv0", "ttb_layernorm_act", "ttb_argmax_rows", "ttb_ar_sample_typical",
 ]
 
 
@@ -281,6 +281,15 @@ def ar_sample(logits, ld_logits, V, B, uniforms, ld_u, seen, codes, ld_codes, fi
     _chk(load().ttb_ar_sample(_p(_f32(logits)), ld_logits, V, B, _p(_f32(uniforms)), ld_u, _p(seen), _p(codes), ld_codes,
                               _p(finished), _p(state), C.c_float(temperature), top_k, C.c_float(top_p),
                               C.c_float(rep_penalty), stop_token, 1 if advance else 0, _stream()), "ttb_ar_sample")
+
+
+def ar_sample_typical(logits, ld_logits, V, B, uniforms, ld_u, seen, codes, ld_codes, finished, state, temperature,
+                      top_k, top_p, rep_penalty, stop_token, typical_mass, advance=True):
+    """ar_sample restricted to the typical set of mass `typical_mass` (in (0, 1]) of the penalised scores."""
+    _chk(load().ttb_ar_sample_typical(_p(_f32(logits)), ld_logits, V, B, _p(_f32(uniforms)), ld_u, _p(seen), _p(codes),
+                                      ld_codes, _p(finished), _p(state), C.c_float(temperature), top_k, C.c_float(top_p),
+                                      C.c_float(rep_penalty), stop_token, 1 if advance else 0, C.c_float(typical_mass),
+                                      _stream()), "ttb_ar_sample_typical")
 
 
 def ar_fix_codes(codes, B, L, stop_token, trim_len):
