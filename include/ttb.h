@@ -50,6 +50,8 @@ typedef struct TtbGemmArgs {
                            (tile_n picks the tile width: 32, 64, else 128); 0/1 = off */
   int variant;          /* 0 = auto; 1 = one tile per CTA; 2 = persistent kernel; with tile_n = 32 also 3 / 4 = one tile
                            per CTA with a 5- / 4-stage pipeline (tools/gemm_sweep.py, tools/gemm_diag.py).
+                           7 = persistent warp-specialised 128x256 kernel, no split-K (the default, unless TTB_GEMM_WS=0,
+                           when tile_n = 0, variant = 0, no split-K / cluster and at least one wave of 128x128 tiles).
                            Experiments not yet validated on hardware (never chosen automatically): 5 = two TMA issuer
                            threads per CTA, 6 = reserved (rejected) */
   float* gn_partials;   /* non-NULL: the epilogue also leaves the GroupNorm statistics of its OUTPUT (after bias, activation

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Times the wgmma GEMM variants (tile width, one-tile-per-CTA vs persistent, cluster multicast, split-K) on the
-shapes of the hot path, next to torch.matmul (cuBLAS) as a calibration of what the hardware delivers on that shape.
-Development aid; prints a table. L2 is flushed between timed launches."""
+"""Times the wgmma GEMM variants (tile width, one-tile-per-CTA vs persistent, the warp-specialised 128x256 kernel, cluster
+multicast, split-K) on the shapes of the hot path, next to torch.matmul (cuBLAS) as a calibration of what the hardware
+delivers on that shape. Development aid; prints a table. L2 is flushed between timed launches."""
 import os
 import sys
 
@@ -72,6 +72,8 @@ def main():
             for cl in (2, 4):
                 if tile != 256 and ((N + tile - 1) // tile) % cl == 0:
                     variants.append(dict(tile_n=tile, cluster=cl))
+        if M > 256:
+            variants.append(dict(variant=7))                   # persistent warp-specialised 128x256 (gemm_ws.cuh)
         if os.environ.get("TTB_TEST_EXPERIMENTAL") == "1" and M > 256:
             variants += [dict(tile_n=128, variant=5)]          # two TMA issuer threads
         if name == "ar proj2":

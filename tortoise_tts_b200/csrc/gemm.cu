@@ -374,6 +374,7 @@ static int launch_tc(const TtbGemmArgs& g, const GemmEpilogue& ep, cudaStream_t 
 
 #include "gemm_persist.cuh"
 #include "gemm_mc.cuh"
+#include "gemm_ws.cuh"
 
 namespace ttb {
 
@@ -418,6 +419,31 @@ static int launch_persistent(const TtbGemmArgs& g, const GemmEpilogue& ep, cudaS
       ma, mb, g.M, g.N, g.K, g.taps, g.pad, (bcast || g.splitk > 1) ? 0 : 1, kb_per_split, m_tiles, n_tiles, zdim, ep);
   if (le != cudaSuccess) return check_cuda(le, "gemm_bf16_tc_persistent_kernel launch");
   TTB_CHECK_LAUNCH("gemm_bf16_tc_persistent_kernel");
+  return 0;
+}
+
+// Persistent warp-specialised 128x256 kernel (gemm_ws.cuh): one CTA per SM, or one per tile when there are fewer.
+static int launch_ws(const TtbGemmArgs& g, const GemmEpilogue& ep, cudaStream_t st) {
+  CUtensorMap ma, mb;
+  const bool bcast = (g.batch == 1) || (g.a_bstride == 0);
+  const uint64_t a_d2 = bcast ? 1 : (uint64_t)g.batch;
+  const uint64_t a_s2 = bcast ? (uint64_t)g.rows * g.lda : (uint64_t)g.a_bstride;
+  if (get_tensor_map_bf16(&ma, g.A, (uint64_t)g.K, (uint64_t)g.rows, a_d2, (uint64_t)g.lda, a_s2, BK, BM)) return -1;
+  if (get_tensor_map_bf16(&mb, g.W, (uint64_t)g.K * g.taps, (uint64_t)g.N, 1, (uint64_t)g.K * g.taps,
+                          (uint64_t)g.K * g.taps * g.N, BK, WS_BN)) return -1;
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_ws_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmWsSmem::TOTAL);
+    if (e != cudaSuccess) return check_cuda(e, "cudaFuncSetAttribute(gemm ws)");
+    attr_set = true;
+  }
+  const int m_tiles = (g.M + BM - 1) / BM, n_tiles = (g.N + WS_BN - 1) / WS_BN;
+  const long long total = (long long)m_tiles * n_tiles * g.batch;
+  const int grid = (int)(total < num_sms() ? total : num_sms());
+  const cudaError_t le = launch_pdl(gemm_bf16_ws_kernel, dim3(grid), dim3(WS_THREADS), (size_t)GemmWsSmem::TOTAL, st,
+      ma, mb, g.M, g.N, g.K, g.taps, g.pad, bcast ? 0 : 1, m_tiles, n_tiles, g.batch, ep);
+  if (le != cudaSuccess) return check_cuda(le, "gemm_bf16_ws_kernel launch");
+  TTB_CHECK_LAUNCH("gemm_bf16_ws_kernel");
   return 0;
 }
 
@@ -493,11 +519,14 @@ extern "C" int ttb_gemm(const TtbGemmArgs* gp, void* stream) {
     return g.cluster == 4 ? launch_mc<128, 3, 4>(g, ep, st) : launch_mc<128, 3, 2>(g, ep, st);
   }
   if (g.variant == 6) { set_error("ttb_gemm: variant 6 (CTA-pair MMA) needs hardware this library does not target"); return -1; }
+  if (g.variant == 7) {
+    if (g.splitk > 1) { set_error("ttb_gemm: variant 7 (warp-specialised 128x256) has no split-K"); return -1; }
+    return launch_ws(g, ep, st);
+  }
   static int persist = -1;   // TTB_GEMM_PERSIST=1 sends problems of >= 2 waves to the persistent kernel (A/B comparison)
   if (persist < 0) { const char* e = getenv("TTB_GEMM_PERSIST"); persist = e ? atoi(e) : 0; }
-  // Off by default: on H100 (80GB HBM3, 700 W) the one-tile kernels were faster on every stage that has several tiles
-  // per SM (standard preset: CLVP 156 -> 118 ms, diffusion 1061 -> 992 ms): the persistent kernel's consumers do not
-  // overlap a tile's epilogue with the next tile's main loop, which co-resident one-tile CTAs do.
+  // Off by default: on H100 (80GB HBM3, 700 W) the 128x128 one-tile kernel was faster than this persistent kernel on
+  // every stage that has several tiles per SM (standard preset: CLVP 156 -> 118 ms, diffusion 1061 -> 992 ms).
   if (g.variant == 2) {
     if (g.tile_n == 32) return launch_persistent<32, 8>(g, ep, st);
     if (g.tile_n == 64) return launch_persistent<64, 6>(g, ep, st);
@@ -510,6 +539,11 @@ extern "C" int ttb_gemm(const TtbGemmArgs* gp, void* stream) {
     if (g.tile_n == 64 || (g.tile_n == 0 && tiles128 < num_sms())) return launch_persistent<64, 6>(g, ep, st);
     if (g.tile_n != 256) return launch_persistent<128, 4>(g, ep, st);
   }
+  // Default for problems of at least one wave of 128x128 tiles: the persistent warp-specialised 128x256 kernel
+  // (gemm_ws.cuh). TTB_GEMM_WS=0 restores the one-tile 128x128 kernel (A/B runs).
+  static int ws = -1;
+  if (ws < 0) { const char* e = getenv("TTB_GEMM_WS"); ws = e ? atoi(e) : 1; }
+  if (ws && g.tile_n == 0 && g.variant == 0 && g.splitk <= 1 && tiles128 >= num_sms()) return launch_ws(g, ep, st);
   if (g.tile_n == 32) {
     // the skinny decode GEMMs are latency-bound (k-block time = TMA round trip / stages): 5 stages still allow two
     // CTAs per SM (2 x 101 KB of the 227 KB). TTB_GEMM_T32_STAGES=4 restores the 4-stage kernel for A/B runs; variant 3 forces 5.

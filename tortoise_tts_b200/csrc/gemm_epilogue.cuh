@@ -10,7 +10,9 @@
 //   * a chunk that is complete (32 columns, 16-byte aligned rows) takes a branch-free FAST path; ragged edges take a
 //     separate, simple per-row SLOW path (lane = row);
 //   * the residual (which may alias the output: x += f(x) in place) is loaded for the whole chunk before any store;
-//   * the tile pitch is BN + 8 floats, so both the fragment stores and the row reads are conflict-free.
+//   * the tile pitch is BN + 8 floats, so both the fragment stores and the row reads are conflict-free (the
+//     warp-specialised kernel stages 32-column slices at pitch 32 to fit two per warpgroup: the row reads stay
+//     conflict-free, the fragment stores become 4-way conflicts).
 #pragma once
 
 namespace ttb {
@@ -21,10 +23,9 @@ TTB_DEVINL float4 lds128(uint32_t addr) {
   return v;
 }
 
-// Accumulator fragments of this thread (rows 64 wg + 16 w + l/4 (+8), see common.cuh) -> fp32 tile [128][BN + 8].
-template <int BN>
+// Accumulator fragments of this thread (rows 64 wg + 16 w + l/4 (+8), see common.cuh) -> fp32 tile [128][PITCH].
+template <int BN, int PITCH = BN + 8>
 TTB_DEVINL void gemm_stage_accumulator(const float* acc, uint32_t tile, int cwarp, int lane) {
-  constexpr int PITCH = BN + 8;
   const uint32_t base = tile + (uint32_t)((cwarp * 16 + (lane >> 2)) * PITCH + 2 * (lane & 3)) * 4;
 #pragma unroll
   for (int i = 0; i < BN / 2; i += 4) {
@@ -172,11 +173,10 @@ TTB_DEVINL void epi_chunk_slow(const uint32_t* r, int nb, int N, int m, int M, l
 
 // One 32-row block of the staged accumulator tile, finished by one warp: `blk` = shared-memory address of the block's
 // first row, chunks ch_begin, ch_begin + ch_step, ... of 32 columns.
-template <int BN, int ACT>
+template <int BN, int ACT, int PITCH = BN + 8>
 TTB_DEVINL void gemm_epilogue_tile(uint32_t blk, int n0, int N, int m_base, int M, int lane, long long bz,
                                    const GemmEpilogue& ep, int ch_begin, int ch_step) {
   constexpr int NCH = BN / 32;
-  constexpr int PITCH = BN + 8;
   const bool aligned = epi_flags(ep).aligned;
   const int rows_valid = min(32, M - m_base);        // warp-uniform; <= 0: this warp's rows are all past M
   // rolled on purpose: one chunk's worth of code and registers
@@ -201,17 +201,17 @@ TTB_DEVINL void gemm_epilogue_tile(uint32_t blk, int n0, int N, int m_base, int 
   }
 }
 
-template <int BN>
+template <int BN, int PITCH = BN + 8>
 TTB_DEVINL void gemm_epilogue_dispatch(uint32_t blk, int n0, int N, int m_base, int M, int lane, long long bz,
                                        const GemmEpilogue& ep, int ch_begin, int ch_step) {
   switch (ep.act) {
-    case TTB_ACT_GEGLU: gemm_epilogue_tile<BN, TTB_ACT_GEGLU>(blk, n0, N, m_base, M, lane, bz, ep, ch_begin, ch_step); break;
-    case TTB_ACT_GELU_NEW: gemm_epilogue_tile<BN, TTB_ACT_GELU_NEW>(blk, n0, N, m_base, M, lane, bz, ep, ch_begin, ch_step); break;
-    case TTB_ACT_SILU: gemm_epilogue_tile<BN, TTB_ACT_SILU>(blk, n0, N, m_base, M, lane, bz, ep, ch_begin, ch_step); break;
-    case TTB_ACT_LRELU02: gemm_epilogue_tile<BN, TTB_ACT_LRELU02>(blk, n0, N, m_base, M, lane, bz, ep, ch_begin, ch_step); break;
-    case TTB_ACT_TANH: gemm_epilogue_tile<BN, TTB_ACT_TANH>(blk, n0, N, m_base, M, lane, bz, ep, ch_begin, ch_step); break;
-    case TTB_ACT_GELU_ERF: gemm_epilogue_tile<BN, TTB_ACT_GELU_ERF>(blk, n0, N, m_base, M, lane, bz, ep, ch_begin, ch_step); break;
-    default: gemm_epilogue_tile<BN, TTB_ACT_NONE>(blk, n0, N, m_base, M, lane, bz, ep, ch_begin, ch_step); break;
+    case TTB_ACT_GEGLU: gemm_epilogue_tile<BN, TTB_ACT_GEGLU, PITCH>(blk, n0, N, m_base, M, lane, bz, ep, ch_begin, ch_step); break;
+    case TTB_ACT_GELU_NEW: gemm_epilogue_tile<BN, TTB_ACT_GELU_NEW, PITCH>(blk, n0, N, m_base, M, lane, bz, ep, ch_begin, ch_step); break;
+    case TTB_ACT_SILU: gemm_epilogue_tile<BN, TTB_ACT_SILU, PITCH>(blk, n0, N, m_base, M, lane, bz, ep, ch_begin, ch_step); break;
+    case TTB_ACT_LRELU02: gemm_epilogue_tile<BN, TTB_ACT_LRELU02, PITCH>(blk, n0, N, m_base, M, lane, bz, ep, ch_begin, ch_step); break;
+    case TTB_ACT_TANH: gemm_epilogue_tile<BN, TTB_ACT_TANH, PITCH>(blk, n0, N, m_base, M, lane, bz, ep, ch_begin, ch_step); break;
+    case TTB_ACT_GELU_ERF: gemm_epilogue_tile<BN, TTB_ACT_GELU_ERF, PITCH>(blk, n0, N, m_base, M, lane, bz, ep, ch_begin, ch_step); break;
+    default: gemm_epilogue_tile<BN, TTB_ACT_NONE, PITCH>(blk, n0, N, m_base, M, lane, bz, ep, ch_begin, ch_step); break;
   }
 }
 
