@@ -140,36 +140,49 @@ def test_step_gemm_and_norm_phases(B, D, H, V, P):
 @pytest.mark.parametrize("B,H,P", [(256, 16, 174), (32, 16, 174), (64, 16, 352), (7, 2, 13)])
 @pytest.mark.parametrize("nc", [1, 7, 8, 9, 16, 17, 33, 215, 429])
 @pytest.mark.parametrize("impl", ["mma", "simt"])
-def test_step_attention_phase(B, H, P, nc, impl, monkeypatch):
+def test_step_attention_phase(B, H, P, nc, impl):
     """Decode attention over [shared prompt prefix | own KV | new token] + the KV append, at `nc` candidate entries
-    (incl. the new one): all chunk-boundary cases of the 16-position ring and the production context lengths."""
-    monkeypatch.setenv("TTB_AR_STEP_ATTN_MMA", "1" if impl == "mma" else "0")   # read at every launch (make_plan)
+    (incl. the new one): all chunk-boundary cases of the 16-position ring and the production context lengths. `impl` is
+    how the candidate's own cache is read: "mma" = the attention phase of the one-kernel step (TMA tiles, mma.sync);
+    "simt" = the per-op decode attention (ttb_ar_decode_attention: SIMT stream over the own cache, prompt part on the
+    tensor cores, merge) on the same inputs, with K and V in separate caches as that path keeps them."""
+    from tortoise_tts_b200 import lib
     D, L, V, Nmax = H * 64, 2, 300, 430
     step = nc                                         # slot = step - 1 = nc - 1 old entries, + the new one
     hd, t = _mk(B, D, H, L, V, P, Nmax, step, seed=nc + B)
     layer = 1
     qkv = t["qkv"].clone()
     kv_before = t["cand_kv"].clone()
-    hd.step(phase_mask=PH_ATTN, layer_begin=layer, layer_end=layer + 1)
-    _check_flag(t)
+    if impl == "mma":
+        hd.step(phase_mask=PH_ATTN, layer_begin=layer, layer_end=layer + 1)
+        _check_flag(t)
+        kv, o = t["cand_kv"], t["o"]
+    else:
+        ck_all, cv_all = kv_before[..., 0, :].contiguous(), kv_before[..., 1, :].contiguous()     # [L][B][H][Nmax][64]
+        pk_l, pv_l = t["prefix_kv"][layer, :, :, 0].contiguous(), t["prefix_kv"][layer, :, :, 1].contiguous()
+        o = torch.empty_like(t["o"])
+        lib.ar_decode_attention(qkv, pk_l, pv_l, ck_all[layer], cv_all[layer], t["state"], B, H, P, Nmax, o,
+                                torch.zeros(2, B, D, device="cuda"), torch.zeros(2, B, H, device="cuda"))
+        _check_flag(t)
+        kv = torch.stack([ck_all, cv_all], dim=-2)
     slot = step - 1
     # the append
-    ck = t["cand_kv"][layer]
+    ck = kv[layer]
     assert torch.equal(ck[:, :, slot, 0], qkv[:, D:2 * D].reshape(B, H, 64))
     assert torch.equal(ck[:, :, slot, 1], qkv[:, 2 * D:].reshape(B, H, 64))
     mask = torch.ones_like(kv_before, dtype=torch.bool)
     mask[layer, :, :, slot] = False
-    assert torch.equal(t["cand_kv"][mask], kv_before[mask]), "attention phase wrote outside the new slot"
+    assert torch.equal(kv[mask], kv_before[mask]), "attention wrote outside the new slot"
     q = qkv[:, :D].reshape(B, H, 1, 64).float() * 0.125
     pk = t["prefix_kv"][layer, :, :, 0].float().unsqueeze(0).expand(B, -1, -1, -1)
     pv = t["prefix_kv"][layer, :, :, 1].float().unsqueeze(0).expand(B, -1, -1, -1)
     K = torch.cat([pk, ck[:, :, :slot + 1, 0].float()], dim=2)
     Vv = torch.cat([pv, ck[:, :, :slot + 1, 1].float()], dim=2)
     want = (torch.softmax(q @ K.transpose(-1, -2), -1) @ Vv).reshape(B, D)
-    r = _rel(t["o"], want)
+    r = _rel(o, want)
     report("ar_step attention %s B=%d P=%d nc=%d" % (impl, B, P, nc), r)
-    # simt: fp32 weights, bf16 store (2^-9). mma: the softmax weights are rounded to bf16 for the P V product, as in every
-    # flash-attention kernel (and in round 1's prompt part): 2^-9 relative on each weight, averaged over the row
+    # mma: the softmax weights are rounded to bf16 for the P V product, as in every flash-attention kernel: 2^-9
+    # relative on each weight, averaged over the row. simt: the same in the prompt part, fp32 weights over the own cache
     assert r < (8e-3 if impl == "mma" else 6e-3)
 
 
@@ -190,7 +203,6 @@ def test_step_matches_per_op_path_and_is_deterministic(B):
     u = torch.rand(B, N)
     runs = {}
     for mode in ("fused", "mixed", "perop"):
-        ar_engine.AREngine.FUSED = 0 if mode == "perop" else 1
         ar_engine.AREngine.MODE = mode
         eng = ar_engine.AREngine(sd, cfg)
         tr = []
@@ -203,7 +215,6 @@ def test_step_matches_per_op_path_and_is_deterministic(B):
             codes_g2 = eng.generate(cond, text, B, N, uniforms=u, use_graph=True).cpu()
             assert torch.equal(codes_g2, codes)
         del eng
-    ar_engine.AREngine.FUSED = int(os.environ.get("TTB_AR_FUSED", "1"))
     ar_engine.AREngine.MODE = os.environ.get("TTB_AR_MODE", "auto")
     # Compare the logits on the common prefix of identical tokens (after the first nucleus-boundary flip the two runs
     # decode different sequences). Scale = the live logits (the synthetic checkpoint pins the stop / start logits at -1e4,

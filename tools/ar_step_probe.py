@@ -35,7 +35,7 @@ def main():
         ts.sort()
         return ts[len(ts) // 2] * 1e3
     names = ["embed+ln1", "c_attn", "attention", "c_proj", "ln_2", "c_fc", "mlp.c_proj", "ln_1'", "mel_head"]
-    print("B=%d step=%d  env: %s" % (B, step, {k: v for k, v in os.environ.items() if k.startswith("TTB_AR_STEP")}))
+    print("B=%d step=%d" % (B, step))
     tot = 0.0
     for i, n in enumerate(names):
         us = timeit(1 << i)

@@ -8,12 +8,13 @@ sd = synth_all(cfg, seed=1, suppress_stop=True)["autoregressive"]
 torch.manual_seed(0)
 text = torch.randint(1, 255, (169,)).tolist() + [0]
 cond = torch.randn(1, cfg.ar_dim)
+default_mode = ar_engine.AREngine.MODE
 for B in (256, 32, 3):
     N = 20
     u = torch.rand(B, N)
     runs = {}
     for fused in (1, 0, 1):
-        ar_engine.AREngine.FUSED = fused
+        ar_engine.AREngine.MODE = default_mode if fused else "perop"
         eng = ar_engine.AREngine(sd, cfg)
         tr = []
         codes = eng.generate(cond, text, B, N, uniforms=u, trace_logits=tr).cpu()

@@ -55,34 +55,27 @@ class AREngine:
         self._dec = None  # decode workspace keyed by (B, P, Nmax)
 
     import os as _os
-    DECODE_CLUSTER = int(_os.environ.get("TTB_AR_CLUSTER", "0"))
-    # TTB_AR_WIDE=1: c_attn / c_fc (N = 3D, 4D: one wave of 64-wide tiles) use 64-column tiles with an 8-stage pipeline
-    DECODE_WIDE = int(_os.environ.get("TTB_AR_WIDE", "0"))
-    # TTB_AR_FUSED=1 (default): the decode step is ONE persistent kernel (csrc/ar_step.cu) + the sampler; 0 = the
-    # per-op CUDA graph (kept as the A/B baseline and for shapes the fused kernel does not cover)
-    FUSED = int(_os.environ.get("TTB_AR_FUSED", "1"))
-    # How the step runs when the one-kernel form is available: "fused" = everything in the persistent kernel, whose
-    # phases grow with the batch (one CTA per SM serialises TMA wait -> MMA -> epilogue inside a phase, which several
-    # small kernels per SM overlap). "mixed" = the per-op graph with its three attention kernels (prefix flash + candidate
-    # stream + merge) replaced by the persistent kernel's attention phase (one launch). "auto" picks by batch size: the
-    # one-kernel step for small batches only (H100 80GB HBM3, 700 W, 256 candidates, 429 steps: AR 1.73 s mixed against
-    # 3.50 s fused; the batch size where the two cross, FUSED_MAX_B, has not been measured on H100).
+    # How the step runs when the one-kernel form (csrc/ar_step.cu) is available: "fused" = everything in the persistent
+    # kernel, whose phases grow with the batch (one CTA per SM serialises TMA wait -> MMA -> epilogue inside a phase,
+    # which several small kernels per SM overlap). "mixed" = the per-op graph with its three attention kernels (prefix
+    # flash + candidate stream + merge) replaced by the persistent kernel's attention phase (one launch). "auto" picks by
+    # batch size: the one-kernel step for small batches only (H100 80GB HBM3, 700 W, 256 candidates, 429 steps: AR 1.73 s
+    # mixed against 3.50 s fused; the batch size where the two cross, FUSED_MAX_B, has not been measured on H100).
+    # "perop" = one kernel per operation: the tests' reference, and the only form for shapes the one-kernel form does not
+    # cover (lib.ar_step_supported).
     MODE = _os.environ.get("TTB_AR_MODE", "auto")            # auto | fused | mixed | perop
     FUSED_MAX_B = int(_os.environ.get("TTB_AR_FUSED_MAX_B", "16"))
     # TTB_AR_CHAINS=2: in mixed mode the candidates are decoded as TWO independent half-batches on two streams inside
     # one captured step. Every kernel of the chain LN -> c_attn -> attention -> c_proj -> LN -> c_fc -> mlp.c_proj is
     # bound by its own latency except the attention (HBM-bound), so the chain of one half fills the bubbles of the
     # other; the attention then runs in compact CTAs (lib.ArStep attn_compact) that leave room for a GEMM CTA per SM.
-    # which decode GEMMs may fetch their weights ahead of griddepcontrol.wait (TtbGemmArgs.w_static): "ln" = the ones that
-    # follow a LayerNorm (which triggers its dependents early), "all", "none"
-    WSTATIC = _os.environ.get("TTB_AR_WSTATIC", "ln")
     # measured on H100 (80GB HBM3, 700 W) at 256 candidates: AR 1839 ms with one chain, 1727 ms with two; split-K 2 / 4
-    # against none: 1727 against 1795 ms; weight prefetch ahead of the dependency wait ("ln" against "none"): 1727 / 1731 ms
-    # (inside the run-to-run spread). CHAINS_MIN_B has not been measured on H100.
+    # against none: 1727 against 1795 ms; weight prefetch ahead of the dependency wait on the GEMMs that follow a
+    # LayerNorm against none: 1727 / 1731 ms (inside the run-to-run spread). CHAINS_MIN_B has not been measured on H100.
     CHAINS = int(_os.environ.get("TTB_AR_CHAINS", "2"))
     CHAINS_MIN_B = int(_os.environ.get("TTB_AR_CHAINS_MIN_B", "128"))
-    SPLITK_PROJ = int(_os.environ.get("TTB_AR_SPLITK_PROJ", "2"))     # attn.c_proj (K = D): 32 n-tiles x 2 m-tiles x 2 splits = 128 CTAs at D=1024, B=256
-    SPLITK_PROJ2 = int(_os.environ.get("TTB_AR_SPLITK_PROJ2", "4"))   # mlp.c_proj (K = 4D): 32 x 2 x 4 = 256 CTAs
+    SPLITK_PROJ = 2      # attn.c_proj (K = D): 32 n-tiles x 2 m-tiles x 2 splits = 128 CTAs at D=1024, B=256
+    SPLITK_PROJ2 = 4     # mlp.c_proj (K = 4D): 32 x 2 x 4 = 256 CTAs
 
     @staticmethod
     def _nsplit(kb_total, splitk):
@@ -149,7 +142,7 @@ class AREngine:
             return self._dec
         self._dec = None                  # release the previous workspace (KV caches) before allocating the next
         cfg, D, dev = self.cfg, self.D, self.dev
-        ok = bool(self.FUSED) and lib.ar_step_supported(B, D, self.H, P)
+        ok = lib.ar_step_supported(B, D, self.H, P)
         mode = self.MODE if ok else "perop"
         if mode == "auto":
             mode = "fused" if B <= self.FUSED_MAX_B else "mixed"
@@ -249,39 +242,34 @@ class AREngine:
         # Skinny-M decode (M = B candidates): every GEMM is weight-streaming bound, so the grid is widened with
         # 32-column tiles and, for the two GEMMs that feed the residual stream, split-K; their partial sums, bias and
         # the residual add are folded into the LayerNorm that follows (fixed summation order -> deterministic).
+        # c_attn, c_fc and mel_head follow a LayerNorm, which triggers its dependents early: they fetch their weights
+        # ahead of griddepcontrol.wait (w_static).
         kb = D // 64
-        # thread-block clusters sharing the activation tile by TMA multicast (TTB_AR_CLUSTER=0 disables)
-        cl = self.DECODE_CLUSTER if D % 128 == 0 else 0
         s1 = min(self.SPLITK_PROJ, kb)
         s2 = min(self.SPLITK_PROJ2, 4 * kb)
         pa, pb = st["part_a"], st["part_b"]
-        wide = dict(tile_n=64, variant=3) if (self.DECODE_WIDE and not cl) else dict(tile_n=32)
-        ws_ln, ws_all = self.WSTATIC in ("ln", "all"), self.WSTATIC == "all"
         prev = None   # (partials, nsplit, bias) of the previous layer's mlp.c_proj, folded into the next LayerNorm
         for l, lw in enumerate(self.w.layers):
             if prev is None:
                 lib.layernorm(x, B, D, lw["ln1_g"], lw["ln1_b"], out_bf16=ws["a"])
             else:
                 lib.residual_layernorm(x, B, D, prev[0], prev[1], B * D, prev[2], lw["ln1_g"], lw["ln1_b"], out_bf16=ws["a"])
-            lib.gemm(ws["a"], lw["wqkv"], M=B, N=3 * D, K=D, bias=lw["bqkv"], out_bf16=ws["qkv"], cluster=cl, w_static=ws_ln,
-                     **wide)
+            lib.gemm(ws["a"], lw["wqkv"], M=B, N=3 * D, K=D, bias=lw["bqkv"], out_bf16=ws["qkv"], tile_n=32, w_static=True)
             if hd is not None:
                 hd.step(phase_mask=4, layer_begin=l, layer_end=l + 1)     # attention phase of the persistent kernel
             else:
                 lib.ar_decode_attention(ws["qkv"], st["pk"][l], st["pv"][l], st["ck"][l], st["cv"][l], st["state"], B, H,
                                         P, Nmax, ws["o"], st["att_o"], st["att_lse"])
-            lib.gemm(ws["o"], lw["wproj"], M=B, N=D, K=D, out_f32=pa, outf_bstride=B * D, tile_n=32, splitk=max(s1, 2), cluster=cl,
-                     w_static=ws_all)
+            lib.gemm(ws["o"], lw["wproj"], M=B, N=D, K=D, out_f32=pa, outf_bstride=B * D, tile_n=32, splitk=max(s1, 2))
             lib.residual_layernorm(x, B, D, pa, self._nsplit(kb, max(s1, 2)), B * D, lw["bproj"], lw["ln2_g"], lw["ln2_b"],
                                    out_bf16=ws["a"])
             lib.gemm(ws["a"], lw["wfc"], M=B, N=4 * D, K=D, bias=lw["bfc"], act=lib.ACT_GELU_NEW, out_bf16=ws["h"],
-                     cluster=cl, w_static=ws_ln, **wide)
-            lib.gemm(ws["h"], lw["wproj2"], M=B, N=D, K=4 * D, out_f32=pb, outf_bstride=B * D, tile_n=32, cluster=cl,
-                     splitk=max(s2, 2), w_static=ws_all)
+                     tile_n=32, w_static=True)
+            lib.gemm(ws["h"], lw["wproj2"], M=B, N=D, K=4 * D, out_f32=pb, outf_bstride=B * D, tile_n=32, splitk=max(s2, 2))
             prev = (pb, self._nsplit(4 * kb, max(s2, 2)), lw["bproj2"])
         lib.residual_layernorm(x, B, D, prev[0], prev[1], B * D, prev[2], self.w.lnf_g, self.w.lnf_b, self.w.fn_g,
                                self.w.fn_b, out_bf16=st["hn"])
-        lib.gemm(st["hn"], self.w.w_head, M=B, N=self.V, K=D, bias=self.w.b_head, out_f32=st["logits"], w_static=ws_ln)
+        lib.gemm(st["hn"], self.w.w_head, M=B, N=self.V, K=D, bias=self.w.b_head, out_f32=st["logits"], w_static=True)
         self._sample(sp, st["logits"], self.V, st)
 
     def _sample(self, sp, logits, ld_logits, ch):

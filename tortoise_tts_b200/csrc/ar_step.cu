@@ -16,9 +16,9 @@
 // - for the two GEMMs that feed the residual stream - by the LayerNorm phase that follows.
 // Attention phase: K|V of a candidate are interleaved per position ([pos][K 64 | V 64], 256 B) so one (candidate, head)
 // stream is one contiguous byte range; each warp pulls its stream through a private 2-stage ring of 4 KB shared-memory
-// buffers with cp.async.bulk + mbarrier (no registers held by loads in flight). The shared prompt prefix of the head is
-// staged in shared memory once per CTA and reused by all of its candidates. At small batch several warps split one stream
-// (flash-decoding) and merge through shared memory.
+// buffers with TMA tensor loads + mbarrier (no registers held by loads in flight). The shared prompt prefix of the head
+// is staged in shared memory once per CTA and reused by all of its candidates. At small batch several warps split one
+// stream (flash-decoding) and merge through shared memory.
 #include "common.cuh"
 #include "ttb_internal.h"
 
@@ -33,7 +33,8 @@ constexpr int AS_WARPS = AS_THREADS / 32;
 constexpr int AS_CHUNK_POS = 16;                           // cache positions per ring stage
 constexpr int AS_POS_BYTES = 256;                          // K row (64 bf16) + V row (64 bf16)
 constexpr int AS_CHUNK_BYTES = AS_CHUNK_POS * AS_POS_BYTES;
-constexpr int AS_RING_BYTES = AS_WARPS * 2 * AS_CHUNK_BYTES;     // 128 KB
+constexpr int AS_RING_NS = 2;                              // ring stages per warp
+constexpr int AS_RING_BYTES = AS_WARPS * AS_RING_NS * AS_CHUNK_BYTES;     // 128 KB
 constexpr int AS_PREFIX_BYTES = 88 * 1024;
 constexpr int AS_MAX_P = AS_PREFIX_BYTES / AS_POS_BYTES;         // 352 prompt positions
 constexpr int AS_DATA_BYTES = AS_RING_BYTES + AS_PREFIX_BYTES;   // GEMM pipeline stages alias this region
@@ -44,6 +45,7 @@ constexpr int AS_W_TILE_BYTES = 128 * 64 * 2;
 constexpr int AS_MAX_TILES = 512;                          // ticket counters (row tile x batch tile)
 constexpr int AS_SYNC_BAR_BYTES = 17 * 128;                // barrier epoch line + 16 arrival-counter lines
 constexpr int AS_COMPACT_WARPS = 8;                        // ar_attn_compact_kernel: 256 threads, ~118 KB at P = 174
+constexpr int AS_COMPACT_CTAS = 2;                         // ar_attn_compact_kernel CTAs per SM
 
 enum { G_QKV = 0, G_PROJ = 1, G_FC = 2, G_PROJ2 = 3, G_HEAD = 4 };
 enum { OUT_PARTIAL = 0, OUT_BF16 = 1, OUT_F32 = 2 };
@@ -60,10 +62,6 @@ struct AsParams {
   int B, D, H, L, V, P, Nmax, pos_mode;
   int TB, nbt, nst, stage_bytes;          // batch tile (wgmma N), number of batch tiles, pipeline stages
   int ncph, ipr, team;                    // attention: CTAs per head, items per round, warps per item
-  int prefetch;
-  int sync_mode;                          // grid barrier flavour (TTB_AR_STEP_SYNC): 0 = conservative, 1 = light
-  int ring_cp, ring_ns;                   // attention ring: positions per stage (8 / 16) and stages per warp (2..4)
-  int attn_impl;                          // 1 = tensor-core (mma.sync) scores / PV from TMA-swizzled tiles, 0 = SIMT
   int layer_begin, layer_end, phase_mask; // debug / profiling: subset of the step (phase_mask bit i = phase i of a layer)
   AsGemmShape g[5];
   const CUtensorMap* maps;                // device: [4*L + 1] weight maps, then activation maps a, o, h, hn
@@ -131,13 +129,6 @@ TTB_DEVINL void mbar_wait_to(uint64_t* bar, uint32_t parity, int* err) {
   }
 }
 
-// 1-D bulk copy global -> shared, completion on an mbarrier (bytes: multiple of 16, 16-B aligned both sides)
-TTB_DEVINL void bulk_g2s(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(smem_dst)),
-               "l"(reinterpret_cast<uint64_t>(gsrc)), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
-
 TTB_DEVINL void tma_prefetch_3d(const CUtensorMap* map, int c0, int c1, int c2) {
   asm volatile("cp.async.bulk.prefetch.tensor.3d.L2.global.tile [%0, {%1, %2, %3}];" ::"l"(reinterpret_cast<uint64_t>(map)),
                "r"(c0), "r"(c1), "r"(c2)
@@ -149,7 +140,7 @@ TTB_DEVINL void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0
 struct AsCtrl {                       // lives in the control block of shared memory
   uint64_t full_bar[AS_MAX_STAGES];
   uint64_t empty_bar[AS_MAX_STAGES];
-  uint64_t ring_bar[AS_WARPS][4];
+  uint64_t ring_bar[AS_WARPS][AS_RING_NS];
   uint64_t prefix_bar;
   uint32_t ticket;
   float red[4][AS_WARPS];
@@ -158,7 +149,7 @@ struct AsCtrl {                       // lives in the control block of shared me
 static_assert(sizeof(AsCtrl) <= AS_CTRL_BYTES, "control block too large");
 
 struct AsCtrlCompact {                // control block of ar_attn_compact_kernel: only what the attention phase touches
-  uint64_t ring_bar[AS_COMPACT_WARPS][4];
+  uint64_t ring_bar[AS_COMPACT_WARPS][AS_RING_NS];
   uint64_t prefix_bar;
   float merge[AS_COMPACT_WARPS][68];
 };
@@ -167,7 +158,7 @@ constexpr int AS_CTRL_COMPACT_BYTES = (int)((sizeof(AsCtrlCompact) + 127) & ~siz
 struct AsRole {                       // per-thread pipeline bookkeeping that survives across phases
   int stage;                          // GEMM smem ring position (producer and consumer threads keep identical copies)
   uint32_t phase;
-  uint32_t ring_par[4];               // attention ring parities of this warp
+  uint32_t ring_par[AS_RING_NS];      // attention ring parities of this warp
   uint32_t prefix_par;
   unsigned long long bar_target;      // next grid-barrier target
 };
@@ -181,7 +172,7 @@ constexpr int AS_BAR_STRIDE = 16;          // u64 elements between slots (128 by
 
 TTB_DEVINL void grid_sync(const AsParams& p, AsRole& rl) {
   int* err = &p.state->reserved[0];
-  // generic-proxy writes of this phase must be ordered before async-proxy (TMA / bulk copy) reads of later phases
+  // generic-proxy writes of this phase must be ordered before async-proxy (TMA) reads of later phases
   fence_proxy_async_all();
   __syncthreads();
   rl.bar_target += 1;                     // barrier epoch
@@ -189,8 +180,7 @@ TTB_DEVINL void grid_sync(const AsParams& p, AsRole& rl) {
     const int lane = threadIdx.x;
     if (lane == 0) {
       unsigned long long* slot = p.bar + AS_BAR_STRIDE * (1 + (blockIdx.x % AS_BAR_SLOTS));
-      if (p.sync_mode == 0) { __threadfence(); atomicAdd(slot, 1ULL); }
-      else asm volatile("red.release.gpu.global.add.u64 [%0], 1;" ::"l"(slot) : "memory");
+      asm volatile("red.release.gpu.global.add.u64 [%0], 1;" ::"l"(slot) : "memory");
     }
     if (*reinterpret_cast<volatile int*>(err) == 0) {
       // CTAs mapped to slot `lane`: blockIdx % SLOTS == lane
@@ -209,10 +199,8 @@ TTB_DEVINL void grid_sync(const AsParams& p, AsRole& rl) {
         }
       }
     }
-    if (p.sync_mode == 0) __threadfence();
   }
   __syncthreads();
-  if (p.sync_mode == 0) fence_proxy_async_all();
 }
 
 // block-wide sum over 512 threads; `buf` is one of ctrl.red[i] (callers alternate buffers so one sync per reduction suffices)
@@ -416,194 +404,8 @@ TTB_DEVINL void gemm_phase(const AsParams& p, const AsGemmShape& g, const CUtens
 }
 
 // ------------------------------------------------------------------ attention phase
-struct AttState { float m, l; float acc[8]; };
-
-TTB_DEVINL float as_dot8(const float* q, const uint4& kk) {
-  const float2 f0 = unpack_bf16(kk.x), f1 = unpack_bf16(kk.y), f2 = unpack_bf16(kk.z), f3 = unpack_bf16(kk.w);
-  float d = q[0] * f0.x + q[1] * f0.y + q[2] * f1.x + q[3] * f1.y + q[4] * f2.x + q[5] * f2.y + q[6] * f3.x + q[7] * f3.y;
-  d += __shfl_xor_sync(0xffffffffu, d, 1);
-  d += __shfl_xor_sync(0xffffffffu, d, 2);
-  d += __shfl_xor_sync(0xffffffffu, d, 4);
-  return d;
-}
-
-// CP positions [pos][K|V] at `buf` (shared memory), npos valid. lane = (psub = lane >> 3, dch = lane & 7): position
-// psub + 4u, dims [8 dch, 8 dch + 8). One shared running-max update per call.
-template <int CP>
-TTB_DEVINL void as_chunk(AttState& st, const float* q, const uint8_t* buf, int npos, int psub, int dch) {
-  constexpr int U = CP / 4;
-  uint4 kk[U], vv[U];
-#pragma unroll
-  for (int u = 0; u < U; ++u) {
-    const uint8_t* pp = buf + (psub + 4 * u) * AS_POS_BYTES + dch * 16;
-    kk[u] = *reinterpret_cast<const uint4*>(pp);
-    vv[u] = *reinterpret_cast<const uint4*>(pp + 128);
-    // rows past npos hold stale bytes (possibly NaN patterns): their weight is exactly 0, so V must be finite
-    if (psub + 4 * u >= npos) vv[u] = make_uint4(0, 0, 0, 0);
-  }
-  float s[U];
-  float bm = -INFINITY;
-#pragma unroll
-  for (int u = 0; u < U; ++u) {
-    s[u] = as_dot8(q, kk[u]);
-    s[u] = (psub + 4 * u < npos) ? s[u] : -INFINITY;
-    bm = fmaxf(bm, s[u]);
-  }
-  const float m_new = fmaxf(st.m, bm);
-  const float m_use = (m_new == -INFINITY) ? 0.f : m_new;
-  const float corr = exp2f(st.m - m_use);
-  st.m = m_new;
-  st.l *= corr;
-#pragma unroll
-  for (int d = 0; d < 8; ++d) st.acc[d] *= corr;
-#pragma unroll
-  for (int u = 0; u < U; ++u) {
-    const float pw = exp2f(s[u] - m_use);
-    st.l += pw;
-    const float2 f0 = unpack_bf16(vv[u].x), f1 = unpack_bf16(vv[u].y), f2 = unpack_bf16(vv[u].z), f3 = unpack_bf16(vv[u].w);
-    st.acc[0] += pw * f0.x; st.acc[1] += pw * f0.y; st.acc[2] += pw * f1.x; st.acc[3] += pw * f1.y;
-    st.acc[4] += pw * f2.x; st.acc[5] += pw * f2.y; st.acc[6] += pw * f3.x; st.acc[7] += pw * f3.y;
-  }
-}
-
-TTB_DEVINL void as_merge(AttState& st, float m_o, float l_o, const float* a_o) {
-  const float m_new = fmaxf(st.m, m_o);
-  const float m_use = (m_new == -INFINITY) ? 0.f : m_new;
-  const float c_s = exp2f(st.m - m_use), c_o = exp2f(m_o - m_use);
-  st.l = st.l * c_s + l_o * c_o;
-#pragma unroll
-  for (int d = 0; d < 8; ++d) st.acc[d] = st.acc[d] * c_s + a_o[d] * c_o;
-  st.m = m_new;
-}
-
-template <int CP>
-TTB_DEVINL void attn_phase(const AsParams& p, int layer, uint8_t* data, AsCtrl* ctrl, AsRole& rl) {
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int psub = lane >> 3, dch = lane & 7;
-  int* err = &p.state->reserved[0];
-  const int B = p.B, H = p.H, P = p.P, Nmax = p.Nmax, D = p.H * 64;
-  const int NS = p.ring_ns;
-  constexpr int CHUNK_BYTES = CP * AS_POS_BYTES;
-  const int slot = p.state->step - 1;                  // the token fed at this step lands in cache slot `slot`
-  const int nold = slot;                               // positions already in the candidate cache
-  uint8_t* ring = data + warp * NS * CHUNK_BYTES;
-  uint8_t* prefix_s = data + p.ipr * p.team * NS * CHUNK_BYTES;   // behind the rings of the active warps (host checks the fit)
-  const __nv_bfloat16* pkv_l = p.prefix_kv + (long long)layer * H * P * 128;
-  __nv_bfloat16* ckv_l = p.cand_kv + (long long)layer * B * H * Nmax * 128;
-  const int units = H * p.ncph;
-  for (int u = blockIdx.x; u < units; u += gridDim.x) {
-    const int h = u % H, ci = u / H;
-    const int b_begin = (int)((long long)ci * B / p.ncph), b_end = (int)((long long)(ci + 1) * B / p.ncph);
-    __syncthreads();                                   // prefix buffer / merge scratch of the previous unit are free
-    if (threadIdx.x == 0) {
-      mbar_arrive_expect_tx(&ctrl->prefix_bar, (uint32_t)(P * AS_POS_BYTES));
-      bulk_g2s(prefix_s, pkv_l + (long long)h * P * 128, (uint32_t)(P * AS_POS_BYTES), &ctrl->prefix_bar);
-    }
-    const int sub = warp % p.team;
-    for (int r0 = b_begin; r0 < b_end; r0 += p.ipr) {
-      const int b = r0 + warp / p.team;
-      const bool valid = (warp < p.ipr * p.team) && (b < b_end);
-      AttState st;
-      st.m = -INFINITY; st.l = 0.f;
-#pragma unroll
-      for (int d = 0; d < 8; ++d) st.acc[d] = 0.f;
-      if (valid) {
-        const __nv_bfloat16* qrow = p.qkv + (long long)b * 3 * D + h * 64;
-        float q[8];
-        {
-          const uint4 uq = __ldcg(reinterpret_cast<const uint4*>(qrow) + dch);
-          const float sc = 0.125f * 1.4426950408889634f;   // 1/sqrt(64) and log2(e)
-          const float2 f0 = unpack_bf16(uq.x), f1 = unpack_bf16(uq.y), f2 = unpack_bf16(uq.z), f3 = unpack_bf16(uq.w);
-          q[0] = f0.x * sc; q[1] = f0.y * sc; q[2] = f1.x * sc; q[3] = f1.y * sc;
-          q[4] = f2.x * sc; q[5] = f2.y * sc; q[6] = f3.x * sc; q[7] = f3.y * sc;
-        }
-        __nv_bfloat16* cb = ckv_l + ((long long)b * H + h) * Nmax * 128;
-        const uint4 k_new = __ldcg(reinterpret_cast<const uint4*>(qrow + D) + dch);
-        const uint4 v_new = __ldcg(reinterpret_cast<const uint4*>(qrow + 2 * D) + dch);
-        // ---- the candidate's own cache, through this warp's ring (chunks sub, sub + team, ...)
-        const int nch = (nold + CP - 1) / CP;
-        if (lane == 0) {
-          for (int s = 0; s < NS; ++s) {
-            const int c = sub + s * p.team;
-            if (c < nch) {
-              const int np = min(CP, nold - c * CP);
-              mbar_arrive_expect_tx(&ctrl->ring_bar[warp][s], (uint32_t)(np * AS_POS_BYTES));
-              bulk_g2s(ring + s * CHUNK_BYTES, cb + (long long)c * CP * 128, (uint32_t)(np * AS_POS_BYTES), &ctrl->ring_bar[warp][s]);
-            }
-          }
-        }
-        if (sub == 0) {
-          // append the new K / V rows (lanes 0-7: K chunks, 8-15: V chunks) and account for them from registers
-          if (lane < 16) reinterpret_cast<uint4*>(cb + (long long)slot * 128 + (lane < 8 ? 0 : 64))[dch] = (lane < 8) ? k_new : v_new;
-          const float s_new = as_dot8(q, k_new);
-          if (psub == 0) {
-            st.m = s_new; st.l = 1.f;
-            const float2 f0 = unpack_bf16(v_new.x), f1 = unpack_bf16(v_new.y), f2 = unpack_bf16(v_new.z), f3 = unpack_bf16(v_new.w);
-            st.acc[0] = f0.x; st.acc[1] = f0.y; st.acc[2] = f1.x; st.acc[3] = f1.y;
-            st.acc[4] = f2.x; st.acc[5] = f2.y; st.acc[6] = f3.x; st.acc[7] = f3.y;
-          }
-        }
-        int s = 0;
-        for (int c_use = sub; c_use < nch; c_use += p.team) {
-          mbar_wait_to(&ctrl->ring_bar[warp][s], rl.ring_par[s], err);
-          rl.ring_par[s] ^= 1;
-          const int np = min(CP, nold - c_use * CP);
-          as_chunk<CP>(st, q, ring + s * CHUNK_BYTES, np, psub, dch);
-          __syncwarp();
-          const int c_next = c_use + NS * p.team;
-          if (lane == 0 && c_next < nch) {
-            const int np2 = min(CP, nold - c_next * CP);
-            mbar_arrive_expect_tx(&ctrl->ring_bar[warp][s], (uint32_t)(np2 * AS_POS_BYTES));
-            bulk_g2s(ring + s * CHUNK_BYTES, cb + (long long)c_next * CP * 128, (uint32_t)(np2 * AS_POS_BYTES), &ctrl->ring_bar[warp][s]);
-          }
-          if (++s == NS) s = 0;
-        }
-        // ---- the shared prompt prefix of this head, from shared memory
-        mbar_wait_to(&ctrl->prefix_bar, rl.prefix_par, err);
-        const int npc = (P + 15) / 16;
-        for (int c = sub; c < npc; c += p.team)
-          as_chunk<16>(st, q, prefix_s + c * 16 * AS_POS_BYTES, min(16, P - c * 16), psub, dch);
-        // ---- merge the 4 position sub-streams of the warp
-#pragma unroll
-        for (int off = 8; off <= 16; off <<= 1) {
-          const float m_o = __shfl_xor_sync(0xffffffffu, st.m, off);
-          const float l_o = __shfl_xor_sync(0xffffffffu, st.l, off);
-          float a_o[8];
-#pragma unroll
-          for (int d = 0; d < 8; ++d) a_o[d] = __shfl_xor_sync(0xffffffffu, st.acc[d], off);
-          as_merge(st, m_o, l_o, a_o);
-        }
-      }
-      if (p.team > 1) {
-        if (valid && psub == 0) {
-          float* ms = ctrl->merge[warp];
-#pragma unroll
-          for (int d = 0; d < 8; ++d) ms[dch * 8 + d] = st.acc[d];
-          if (dch == 0) { ms[64] = st.m; ms[65] = st.l; }
-        }
-        __syncthreads();
-        if (valid && sub == 0 && psub == 0) {
-          for (int t = 1; t < p.team; ++t) {
-            const float* ms = ctrl->merge[warp + t];
-            as_merge(st, ms[64], ms[65], ms + dch * 8);
-          }
-        }
-      }
-      if (valid && sub == 0 && psub == 0) {
-        const float inv = 1.0f / st.l;
-        uint4 o4 = make_uint4(pack_bf16(st.acc[0] * inv, st.acc[1] * inv), pack_bf16(st.acc[2] * inv, st.acc[3] * inv),
-                              pack_bf16(st.acc[4] * inv, st.acc[5] * inv), pack_bf16(st.acc[6] * inv, st.acc[7] * inv));
-        reinterpret_cast<uint4*>(p.o + (long long)b * D + h * 64)[dch] = o4;
-      }
-      if (p.team > 1) __syncthreads();                 // merge scratch is rewritten by the next round
-    }
-    rl.prefix_par ^= 1;
-  }
-}
-
-// ------------------------------------------------------------------ attention phase, tensor-core form
-// The SIMT form above spends ~14 issue slots per cached position (bf16 unpacking, 8-lane dot products, shuffles): at 256
-// candidates the phase is issue-bound rather than bound by its KV traffic, and the shared prompt part is a large share of it.
+// A SIMT form spends ~14 issue slots per cached position (bf16 unpacking, 8-lane dot products, shuffles): at 256
+// candidates it is issue-bound rather than bound by its KV traffic, and the shared prompt part is a large share of it.
 // Here both products of a 16-position chunk run on the tensor cores (mma.sync m16n8k16, bf16 in / fp32 out):
 //   S[16 pos] = K[16 x 64] q      : A = K chunk (row = position), B = q in column 0 of the 16 x 8 operand
 //   O[64]    += V^T[64 x 16] p    : A = V chunk read transposed (ldmatrix.trans), B = p (bf16) in column 0
@@ -688,12 +490,12 @@ TTB_DEVINL void attn_phase_mma(const AsParams& p, int layer, uint8_t* data, Ctrl
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   int* err = &p.state->reserved[0];
   const int B = p.B, H = p.H, P = p.P, Nmax = p.Nmax, D = p.H * 64;
-  const int NS = p.ring_ns;
-  constexpr int CHUNK_BYTES = 16 * AS_POS_BYTES;       // K tile 2 KB | V tile 2 KB
+  constexpr int NS = AS_RING_NS;
+  constexpr int CHUNK_BYTES = AS_CHUNK_BYTES;          // K tile 2 KB | V tile 2 KB
   const int slot = p.state->step - 1;
   const int nold = slot;
   uint8_t* ring = data + warp * NS * CHUNK_BYTES;
-  uint8_t* prefix_s = data + p.ipr * p.team * NS * CHUNK_BYTES;
+  uint8_t* prefix_s = data + p.ipr * p.team * NS * CHUNK_BYTES;   // behind the rings of the active warps (host checks the fit)
   const CUtensorMap* map_c = p.maps + 4 * p.L + 5;
   const CUtensorMap* map_p = map_c + 1;
   __nv_bfloat16* ckv_l = p.cand_kv + (long long)layer * B * H * Nmax * 128;
@@ -715,18 +517,13 @@ TTB_DEVINL void attn_phase_mma(const AsParams& p, int layer, uint8_t* data, Ctrl
     // first NS tiles of candidate bb's stream into this warp's ring (lane 0). All stages are free whenever this is
     // called: at the start of the unit, or after the last tile of the previous item was consumed.
     auto issue_head = [&](int bb) {
-      const __nv_bfloat16* cbb = ckv_l + ((long long)bb * H + h) * Nmax * 128;
       const int it = (layer * B + bb) * H + h;
       for (int s = 0; s < NS; ++s) {
         const int c = sub + s * p.team;
         if (c < nch) {
           mbar_arrive_expect_tx(&ctrl->ring_bar[warp][s], (uint32_t)CHUNK_BYTES);
-          if (p.attn_impl == 2) {
-            bulk_g2s(ring + s * CHUNK_BYTES, cbb + (long long)c * 16 * 128, (uint32_t)CHUNK_BYTES, &ctrl->ring_bar[warp][s]);
-          } else {
-            tma_load_4d(ring + s * CHUNK_BYTES, map_c, &ctrl->ring_bar[warp][s], 0, 0, c * 16, it);
-            tma_load_4d(ring + s * CHUNK_BYTES + 2048, map_c, &ctrl->ring_bar[warp][s], 0, 1, c * 16, it);
-          }
+          tma_load_4d(ring + s * CHUNK_BYTES, map_c, &ctrl->ring_bar[warp][s], 0, 0, c * 16, it);
+          tma_load_4d(ring + s * CHUNK_BYTES + 2048, map_c, &ctrl->ring_bar[warp][s], 0, 1, c * 16, it);
         }
       }
     };
@@ -799,12 +596,8 @@ TTB_DEVINL void attn_phase_mma(const AsParams& p, int layer, uint8_t* data, Ctrl
           const int c_next = c_use + NS * p.team;
           if (lane == 0 && c_next < nch) {
             mbar_arrive_expect_tx(&ctrl->ring_bar[warp][s], (uint32_t)CHUNK_BYTES);
-            if (p.attn_impl == 2) {
-              bulk_g2s(ring + s * CHUNK_BYTES, cb + (long long)c_next * 16 * 128, (uint32_t)CHUNK_BYTES, &ctrl->ring_bar[warp][s]);
-            } else {
-              tma_load_4d(ring + s * CHUNK_BYTES, map_c, &ctrl->ring_bar[warp][s], 0, 0, c_next * 16, item);
-              tma_load_4d(ring + s * CHUNK_BYTES + 2048, map_c, &ctrl->ring_bar[warp][s], 0, 1, c_next * 16, item);
-            }
+            tma_load_4d(ring + s * CHUNK_BYTES, map_c, &ctrl->ring_bar[warp][s], 0, 0, c_next * 16, item);
+            tma_load_4d(ring + s * CHUNK_BYTES + 2048, map_c, &ctrl->ring_bar[warp][s], 0, 1, c_next * 16, item);
           }
           if (++s == NS) s = 0;
         }
@@ -945,7 +738,7 @@ __global__ void __launch_bounds__(AS_THREADS, 1) ar_step_kernel(const __grid_con
   if (warp == 0 && lane == 0) {
     for (int s = 0; s < AS_MAX_STAGES; ++s) { mbar_init(&ctrl->full_bar[s], 1); mbar_init(&ctrl->empty_bar[s], 2); }
     for (int w = 0; w < AS_WARPS; ++w)
-      for (int k = 0; k < 4; ++k) mbar_init(&ctrl->ring_bar[w][k], 1);
+      for (int k = 0; k < AS_RING_NS; ++k) mbar_init(&ctrl->ring_bar[w][k], 1);
     mbar_init(&ctrl->prefix_bar, 1);
     fence_barrier_init();
   }
@@ -953,14 +746,14 @@ __global__ void __launch_bounds__(AS_THREADS, 1) ar_step_kernel(const __grid_con
 
   AsRole rl;
   rl.stage = 0; rl.phase = 0; rl.prefix_par = 0;
-  rl.ring_par[0] = rl.ring_par[1] = rl.ring_par[2] = rl.ring_par[3] = 0;
+  rl.ring_par[0] = rl.ring_par[1] = 0;
   rl.bar_target = ld_acquire_u64(p.bar);          // barrier epoch at launch (bar[0]; the arrival slots follow)
 
   const CUtensorMap* map_a = p.maps + 4 * p.L + 1;
   const CUtensorMap* map_o = map_a + 1;
   const CUtensorMap* map_h = map_a + 2;
   const CUtensorMap* map_hn = map_a + 3;
-  const bool pf = p.prefetch && warp == 2 && lane == 0;
+  const bool pf = warp == 2 && lane == 0;            // L2 prefetch of the next phases' weight tiles
   const int L0 = p.layer_begin, L1 = p.layer_end;
   // the barrier behind the last phase of the launch orders nothing (the kernel boundary does): skip it
   int last_bit = 0;
@@ -984,9 +777,7 @@ __global__ void __launch_bounds__(AS_THREADS, 1) ar_step_kernel(const __grid_con
       AS_SYNC_UNLESS_LAST(1, l);
     }
     if (p.phase_mask & PH_ATTN) {
-      if (p.attn_impl >= 1) attn_phase_mma(p, l, data, ctrl, rl);
-      else if (p.ring_cp == 8) attn_phase<8>(p, l, data, ctrl, rl);
-      else attn_phase<16>(p, l, data, ctrl, rl);
+      attn_phase_mma(p, l, data, ctrl, rl);
       AS_SYNC_UNLESS_LAST(2, l);
     }
     if (p.phase_mask & PH_NOP) grid_sync(p, rl);
@@ -1038,20 +829,15 @@ __global__ void __launch_bounds__(AS_THREADS, 1) ar_attn_only_kernel(const __gri
   AsCtrl* ctrl = reinterpret_cast<AsCtrl*>(data + AS_DATA_BYTES);
   if (threadIdx.x == 0) {
     for (int w = 0; w < AS_WARPS; ++w)
-      for (int k = 0; k < 4; ++k) mbar_init(&ctrl->ring_bar[w][k], 1);
+      for (int k = 0; k < AS_RING_NS; ++k) mbar_init(&ctrl->ring_bar[w][k], 1);
     mbar_init(&ctrl->prefix_bar, 1);
     fence_barrier_init();
   }
   __syncthreads();
-  if (p.attn_impl < 1) pdl_wait();  // qkv belongs to the c_attn GEMM before this point (TTB_PDL=1); the tensor-core form
-                                    // waits inside, after it has requested its first cache tiles
   AsRole rl;
   rl.stage = 0; rl.phase = 0; rl.prefix_par = 0; rl.bar_target = 0;
-  rl.ring_par[0] = rl.ring_par[1] = rl.ring_par[2] = rl.ring_par[3] = 0;
-  const int l = p.layer_begin;
-  if (p.attn_impl >= 1) attn_phase_mma(p, l, data, ctrl, rl, true);
-  else if (p.ring_cp == 8) attn_phase<8>(p, l, data, ctrl, rl);
-  else attn_phase<16>(p, l, data, ctrl, rl);
+  rl.ring_par[0] = rl.ring_par[1] = 0;
+  attn_phase_mma(p, p.layer_begin, data, ctrl, rl, true);   // waits for the c_attn GEMM (PDL) after its first requests
   pdl_launch_dependents();
 }
 
@@ -1061,20 +847,20 @@ __global__ void __launch_bounds__(AS_THREADS, 1) ar_attn_only_kernel(const __gri
 // (prompts up to 176 positions), which gives the SM its 16 concurrent KV streams back when the kernel has it to itself. Used when the candidates are decoded
 // as two independent half-batches on two streams (ar_engine.py, TTB_AR_CHAINS): the latency-bound GEMM / LayerNorm
 // chain of one half then overlaps the bandwidth-bound attention of the other.
-__global__ void __launch_bounds__(AS_COMPACT_WARPS * 32, 2) ar_attn_compact_kernel(const __grid_constant__ AsParams p) {
+__global__ void __launch_bounds__(AS_COMPACT_WARPS * 32, AS_COMPACT_CTAS) ar_attn_compact_kernel(const __grid_constant__ AsParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* data = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   AsCtrlCompact* ctrl = reinterpret_cast<AsCtrlCompact*>(data + p.attn_data_bytes);
   if (threadIdx.x == 0) {
     for (int w = 0; w < AS_COMPACT_WARPS; ++w)
-      for (int k = 0; k < 4; ++k) mbar_init(&ctrl->ring_bar[w][k], 1);
+      for (int k = 0; k < AS_RING_NS; ++k) mbar_init(&ctrl->ring_bar[w][k], 1);
     mbar_init(&ctrl->prefix_bar, 1);
     fence_barrier_init();
   }
   __syncthreads();
   AsRole rl;
   rl.stage = 0; rl.phase = 0; rl.prefix_par = 0; rl.bar_target = 0;
-  rl.ring_par[0] = rl.ring_par[1] = rl.ring_par[2] = rl.ring_par[3] = 0;
+  rl.ring_par[0] = rl.ring_par[1] = 0;
   attn_phase_mma(p, p.layer_begin, data, ctrl, rl, true);
   pdl_launch_dependents();
 }
@@ -1096,7 +882,6 @@ struct AsPlan {
   AsParams p;
   long long part_floats;
   int grid;
-  int compact_ctas;      // CTAs per SM the compact attention launch is sized for
 };
 
 static int as_num_sms() {
@@ -1131,9 +916,7 @@ static int make_plan(const TtbArStepArgs& a, AsPlan& pl) {
   if (a.D != a.H * 64 || a.D % 128 != 0 || a.D > 1024) { set_error("ttb_ar_step: D=%d H=%d unsupported (D = 64 H, D %% 128 == 0, D <= 1024)", a.D, a.H); return -1; }
   if (a.P <= 0 || a.P > AS_MAX_P) { set_error("ttb_ar_step: prompt length P=%d exceeds %d", a.P, AS_MAX_P); return -1; }
   if (a.L <= 0 || a.V <= 0 || a.Nmax <= 0) { set_error("ttb_ar_step: bad shape"); return -1; }
-  int grid = as_num_sms();
-  const int gcap = env_int("TTB_AR_STEP_GRID", 0);
-  if (gcap > 0 && gcap < grid) grid = gcap;
+  const int grid = as_num_sms();
   pl.grid = grid;
   p.B = a.B; p.D = a.D; p.H = a.H; p.L = a.L; p.V = a.V; p.P = a.P; p.Nmax = a.Nmax; p.pos_mode = a.pos_mode;
   const int Bpad = (a.B + 15) & ~15;
@@ -1142,8 +925,9 @@ static int make_plan(const TtbArStepArgs& a, AsPlan& pl) {
   p.stage_bytes = AS_W_TILE_BYTES + p.TB * 128;
   p.nst = AS_DATA_BYTES / p.stage_bytes;
   if (p.nst > AS_MAX_STAGES) p.nst = AS_MAX_STAGES;
-  const int cap_f = env_int("TTB_AR_STEP_SPLIT_FINAL", 8);      // try 1 at B > 128: direct epilogue, no fix-up
-  const int cap_p = env_int("TTB_AR_STEP_SPLIT_PART", p.nbt > 1 ? 4 : 8);
+  // most K splits: GEMMs with a final (bf16 / logit) output, and the two whose partials the next LayerNorm sums
+  const int cap_f = 8;
+  const int cap_p = p.nbt > 1 ? 4 : 8;
   plan_gemm(p.g[G_QKV], 3 * a.D, a.D, p.nbt, grid, cap_f);
   plan_gemm(p.g[G_PROJ], a.D, a.D, p.nbt, grid, cap_p);
   plan_gemm(p.g[G_FC], 4 * a.D, a.D, p.nbt, grid, cap_f);
@@ -1156,54 +940,33 @@ static int make_plan(const TtbArStepArgs& a, AsPlan& pl) {
     if (p.g[i].n_rt * p.nbt > AS_MAX_TILES) { set_error("ttb_ar_step: too many tiles"); return -1; }
   }
   pl.part_floats = pf;
-  // attention decomposition
-  // (compact attention: up to two CTAs per SM, see ar_attn_compact_kernel; TTB_AR_COMPACT_CTAS=1 keeps one)
-  pl.compact_ctas = 1;
-  if (a.attn_compact) { pl.compact_ctas = env_int("TTB_AR_COMPACT_CTAS", 2); if (pl.compact_ctas < 1 || pl.compact_ctas > 2) pl.compact_ctas = 2; }
-  p.ncph = grid * pl.compact_ctas / a.H;
+  // attention decomposition (compact attention: AS_COMPACT_CTAS CTAs per SM, see ar_attn_compact_kernel)
+  p.ncph = grid * (a.attn_compact ? AS_COMPACT_CTAS : 1) / a.H;
   if (p.ncph < 1) p.ncph = 1;
   if (p.ncph > a.B) p.ncph = a.B;
   const int max_items = (a.B + p.ncph - 1) / p.ncph;
-  int wcap = env_int("TTB_AR_STEP_ATTN_WARPS", AS_WARPS);      // experiments: fewer concurrent streams, deeper rings
-  if (wcap < 1 || wcap > AS_WARPS) wcap = AS_WARPS;
-  if (a.attn_compact && wcap > AS_COMPACT_WARPS) wcap = AS_COMPACT_WARPS;
+  const int wcap = a.attn_compact ? AS_COMPACT_WARPS : AS_WARPS;
   const int rounds = (max_items + wcap - 1) / wcap;
   p.ipr = (max_items + rounds - 1) / rounds;
   int team = 1;
   while (team * 2 * p.ipr <= wcap) team *= 2;
+  // test hook: TTB_AR_STEP_TEAM caps the warps per stream, so that runs at different batch sizes merge the same way
+  // (test_two_chains_match_one_chain compares them bit for bit)
   const int tcap = env_int("TTB_AR_STEP_TEAM", 0);
   if (tcap > 0 && tcap < team) team = tcap;
   p.team = team;
-  p.prefetch = env_int("TTB_AR_STEP_PREFETCH", 1);
-  p.sync_mode = env_int("TTB_AR_STEP_SYNC", 1);
-  p.attn_impl = env_int("TTB_AR_STEP_ATTN_MMA", 1);      // 0 SIMT, 1 tensor-core, 2 = 1 with bulk-copy fills (timing only)
-  if (p.attn_impl < 0 || p.attn_impl > 2) p.attn_impl = 1;
-  p.ring_cp = (env_int("TTB_AR_STEP_RING_CP", 16) == 8 && p.attn_impl == 0) ? 8 : 16;
-  p.ring_ns = env_int("TTB_AR_STEP_RING_NS", 2);
-  if (p.ring_ns < 2) p.ring_ns = 2;
-  if (p.ring_ns > 4) p.ring_ns = 4;
   // the rings of the active warps + the prompt prefix of one head share the data region
-  {
-    const int nact = p.ipr * p.team;
-    const long long pref = (long long)((a.P + 15) & ~15) * AS_POS_BYTES;
-    while (p.ring_ns > 2 && (long long)nact * p.ring_ns * p.ring_cp * AS_POS_BYTES + pref > AS_DATA_BYTES) --p.ring_ns;
-    if ((long long)nact * p.ring_ns * p.ring_cp * AS_POS_BYTES + pref > AS_DATA_BYTES) {
-      set_error("ttb_ar_step: ring %d x %d positions x %d warps + prompt %d do not fit shared memory", p.ring_ns, p.ring_cp,
-                nact, a.P);
-      return -1;
-    }
+  const int nact = p.ipr * p.team;
+  const long long attn_bytes = (long long)nact * AS_RING_NS * AS_CHUNK_BYTES + (long long)((a.P + 15) & ~15) * AS_POS_BYTES;
+  if (attn_bytes > AS_DATA_BYTES) {
+    set_error("ttb_ar_step: ring %d x %d positions x %d warps + prompt %d do not fit shared memory", AS_RING_NS, AS_CHUNK_POS,
+              nact, a.P);
+    return -1;
   }
-  p.attn_data_bytes = 0;
-  if (a.attn_compact) {
-    p.ring_ns = 2;
-    const long long need = (long long)p.ipr * p.team * p.ring_ns * p.ring_cp * AS_POS_BYTES + (long long)((a.P + 15) & ~15) * AS_POS_BYTES;
-    p.attn_data_bytes = (int)((need + 1023) & ~1023LL);
-  }
+  p.attn_data_bytes = a.attn_compact ? (int)((attn_bytes + 1023) & ~1023LL) : 0;
   p.layer_begin = 0; p.layer_end = a.L; p.phase_mask = 0x1ff;
   if (a.debug_layer_end > 0) { p.layer_begin = a.debug_layer_begin; p.layer_end = a.debug_layer_end; }
   if (a.debug_phase_mask) p.phase_mask = a.debug_phase_mask;
-  const int pcap = env_int("TTB_AR_STEP_PROJ2_SPLIT", 0);      // experiments: split count of mlp.c_proj alone
-  if (pcap > 0) plan_gemm(p.g[G_PROJ2], a.D, 4 * a.D, p.nbt, grid, pcap);
   return 0;
 }
 
@@ -1303,8 +1066,7 @@ extern "C" int ttb_ar_decode_step(const TtbArStepArgs* ap, void* stream) {
   if (p.phase_mask == PH_ATTN && p.layer_end == p.layer_begin + 1) {
     const int units = a.H * p.ncph;
     if (a.attn_compact) {
-      if (p.attn_impl < 1) { set_error("ttb_ar_decode_step: attn_compact needs the tensor-core attention"); return -1; }
-      const int cgrid = pl.grid * pl.compact_ctas;
+      const int cgrid = pl.grid * AS_COMPACT_CTAS;
       const cudaError_t lc = launch_pdl(ar_attn_compact_kernel, dim3(units < cgrid ? units : cgrid), dim3(AS_COMPACT_WARPS * 32),
                                         (size_t)(p.attn_data_bytes + AS_CTRL_COMPACT_BYTES + 1024), st, p);
       if (lc != cudaSuccess) return check_cuda(lc, "ar_attn_compact_kernel launch");
