@@ -97,7 +97,11 @@ int ttb_rmsnorm(const float* x, int M, int D, const float* g, void* out_bf16, vo
  * row *ss_row (device-side step counter) at stride ss_row_stride is used); if silu: y = SiLU(y).
  * `partials` is a scratch buffer of TTB_GROUPNORM_SCRATCH_FLOATS(B, groups) floats (per-block partial sums between
  * the statistics and the apply kernel; nothing is kept across calls, so one buffer may serve any number of calls on
- * the same stream). Results are bit-reproducible (no atomics). Output bf16 [B, S, ldo] and/or fp32. */
+ * the same stream). Results are bit-reproducible (no atomics). Output bf16 [B, S, ldo] and/or fp32.
+ * Channels per group: a multiple of 4, or exactly 2. The 2-per-group form is GN(16 groups, C = 32) of the
+ * tortoise-detect classifier's first level (models/classifier.py, normalization() at arch_util.py:26-41); it needs
+ * C / 4 a power of two <= 256, no scale_shift, and ldo / ldof multiples of 4 (columns C..ldo-1 are not written).
+ * Anything else returns an error. */
 #define TTB_GROUPNORM_SPLITS 128
 #define TTB_GROUPNORM_SCRATCH_FLOATS(B, groups) ((B) * (groups) * (2 * TTB_GROUPNORM_SPLITS + 2) + 16)
 int ttb_groupnorm(const float* x, int B, int S, int C, int groups, const float* gamma, const float* beta,

@@ -159,9 +159,29 @@ def _typical_mass(typical_sampling, typical_mass):
     return m
 
 
-def classify_audio_clip(clip):
-    """api.py:133-145 (AudioMiniEncoderWithClassifierHead): not on the synthesis path; out of scope (SURVEY §8f-4)."""
-    raise NotImplementedError("classify_audio_clip is outside the hot path this engine replaces (SURVEY §8f-4)")
+_CLASSIFIERS = {}
+
+
+def classify_audio_clip(clip, models_dir=MODELS_DIR):
+    """≙ api.py:133-145: the probability that the tortoise-detect classifier (AudioMiniEncoderWithClassifierHead)
+    assigns to class 0 of `clip`, a [1, n] float waveform at 24 kHz on any device, as a 0-d float32 CPU tensor
+    (softmax(logits)[0][0]). Any other shape raises ValueError.
+
+    Deliberate differences: the classifier runs on the current CUDA device (classifier_engine.py), not on the CPU; and
+    `classifier.pth` is loaded on the first call and the packed engine is kept per (checkpoint path, device), where the
+    reference reloads the checkpoint on every call."""
+    if not torch.is_tensor(clip) or clip.dim() != 2 or clip.shape[0] != 1 or clip.shape[1] < 1 \
+            or not clip.is_floating_point():
+        raise ValueError("classify_audio_clip expects a float waveform of shape [1, n], got %s" %
+                         ((tuple(clip.shape) if torch.is_tensor(clip) else type(clip).__name__),))
+    from .classifier_engine import ClassifierEngine
+    path = os.path.abspath(get_model_path("classifier.pth", models_dir))
+    dev = torch.device("cuda", torch.cuda.current_device())
+    eng = _CLASSIFIERS.get((path, dev))
+    if eng is None:
+        eng = _CLASSIFIERS[(path, dev)] = ClassifierEngine(torch.load(path, map_location="cpu", weights_only=True), dev)
+    _, probs = eng.forward(clip)
+    return probs[0, 0].cpu()
 
 
 def pick_best_batch_size_for_gpu():

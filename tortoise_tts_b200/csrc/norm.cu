@@ -370,6 +370,111 @@ gn_apply_rows_kernel(const float* __restrict__ x, int S, int C, int groups, int 
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Row-wise GroupNorm with 2 channels per group: the level-0 ResBlocks of the tortoise-detect classifier (C = 32,
+// normalization() gives 16 groups; models/classifier.py, arch_util.py:26-41), S = the clip's samples. Same block
+// structure as the row-wise kernels above, but a thread's float4 holds two whole groups, so a thread keeps two
+// (sum, sumsq) pairs and no lanes share a group. Same statistic and scratch layout: one (sum, sumsq) partial per
+// (batch, group, block), folded in a fixed order; no atomics.
+__global__ void __launch_bounds__(256)
+gn_stats_pairs_kernel(const float* __restrict__ x, int S, int C, int groups, int tpr, int rows_per,
+                      float* __restrict__ scratch) {
+  pdl_wait();
+  __shared__ float sacc[1024];                                  // [row lane][group][2]: (256 / tpr) * (2 * tpr) * 2
+  const int sp = blockIdx.x, b = blockIdx.y;
+  const int rows_par = 256 / tpr;
+  const int rl = threadIdx.x / tpr, ct = threadIdx.x - rl * tpr;
+  const int s0 = sp * rows_per, s1 = min(S, s0 + rows_per);
+  const float* xp = x + (long long)b * S * C + ct * 4;
+  float sa = 0.f, qa = 0.f, sb = 0.f, qb = 0.f;
+  int r = s0 + rl;
+  for (; r + 7 * rows_par < s1; r += 8 * rows_par) {
+    float4 t[8];
+#pragma unroll
+    for (int u = 0; u < 8; ++u) t[u] = *reinterpret_cast<const float4*>(xp + (long long)(r + u * rows_par) * C);
+#pragma unroll
+    for (int u = 0; u < 8; ++u) {
+      sa += t[u].x + t[u].y;
+      qa += t[u].x * t[u].x + t[u].y * t[u].y;
+      sb += t[u].z + t[u].w;
+      qb += t[u].z * t[u].z + t[u].w * t[u].w;
+    }
+  }
+  for (; r < s1; r += rows_par) {
+    const float4 t = *reinterpret_cast<const float4*>(xp + (long long)r * C);
+    sa += t.x + t.y;
+    qa += t.x * t.x + t.y * t.y;
+    sb += t.z + t.w;
+    qb += t.z * t.z + t.w * t.w;
+  }
+  float* sr = sacc + (rl * groups + 2 * ct) * 2;
+  sr[0] = sa; sr[1] = qa; sr[2] = sb; sr[3] = qb;
+  __syncthreads();
+  for (int g = threadIdx.x; g < groups; g += 256) {
+    float su = 0.f, sq = 0.f;
+    for (int k = 0; k < rows_par; ++k) { su += sacc[(k * groups + g) * 2]; sq += sacc[(k * groups + g) * 2 + 1]; }
+    float* p = scratch + 16 + (((long long)b * groups + g) * TTB_GN_SPLITS + sp) * 2;
+    p[0] = su;
+    p[1] = sq;
+  }
+}
+
+__global__ void __launch_bounds__(256)
+gn_apply_pairs_kernel(const float* __restrict__ x, int S, int C, int groups, int tpr, int rows_per, int splits,
+                      const float* __restrict__ scratch, const float* __restrict__ gamma, const float* __restrict__ beta,
+                      int do_silu, __nv_bfloat16* __restrict__ ob, int ldo, float* __restrict__ of, int ldof, int early) {
+  if (early) pdl_launch_dependents();
+  pdl_wait();
+  const int b = blockIdx.y;
+  const int rows_par = 256 / tpr;
+  const int rl = threadIdx.x / tpr, ct = threadIdx.x - rl * tpr;
+  const int c = ct * 4, g = ct * 2;
+  // the lanes of a warp with the same columns (lane bits >= log2 tpr) take every nsh-th partial, then a fixed xor tree
+  const int nsh = tpr < 32 ? 32 / tpr : 1, sub = (threadIdx.x & 31) / tpr;
+  const float2* part = reinterpret_cast<const float2*>(scratch + 16) + ((long long)b * groups + g) * TTB_GN_SPLITS;
+  float sa = 0.f, qa = 0.f, sb = 0.f, qb = 0.f;
+  for (int k = sub; k < splits; k += nsh) {
+    const float2 pa = part[k], pb = part[TTB_GN_SPLITS + k];
+    sa += pa.x; qa += pa.y;
+    sb += pb.x; qb += pb.y;
+  }
+  for (int off = tpr; off < 32; off <<= 1) {
+    sa += __shfl_xor_sync(0xffffffffu, sa, off);
+    qa += __shfl_xor_sync(0xffffffffu, qa, off);
+    sb += __shfl_xor_sync(0xffffffffu, sb, off);
+    qb += __shfl_xor_sync(0xffffffffu, qb, off);
+  }
+  const float n = (float)S * 2.f;
+  const float ma = sa / n, mb = sb / n;
+  const float ra = rsqrtf(fmaxf(qa / n - ma * ma, 0.f) + 1e-5f), rb = rsqrtf(fmaxf(qb / n - mb * mb, 0.f) + 1e-5f);
+  float a[4], o[4];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    a[j] = (j < 2 ? ra : rb) * __ldg(gamma + c + j);
+    o[j] = __ldg(beta + c + j) - (j < 2 ? ma : mb) * a[j];
+  }
+  const int s0 = blockIdx.x * rows_per, s1 = min(S, s0 + rows_per);
+  const float* xp = x + (long long)b * S * C + c;
+  for (int r0 = s0 + rl; r0 < s1; r0 += 8 * rows_par) {
+    float4 t[8];
+#pragma unroll
+    for (int u = 0; u < 8; ++u) {
+      const int r = r0 + u * rows_par;
+      if (r < s1) t[u] = *reinterpret_cast<const float4*>(xp + (long long)r * C);
+    }
+#pragma unroll
+    for (int u = 0; u < 8; ++u) {
+      const int r = r0 + u * rows_par;
+      if (r >= s1) break;
+      float y0 = fmaf(t[u].x, a[0], o[0]), y1 = fmaf(t[u].y, a[1], o[1]), y2 = fmaf(t[u].z, a[2], o[2]),
+            y3 = fmaf(t[u].w, a[3], o[3]);
+      if (do_silu) { y0 = silu(y0); y1 = silu(y1); y2 = silu(y2); y3 = silu(y3); }
+      if (ob) *reinterpret_cast<uint2*>(ob + ((long long)b * S + r) * ldo + c) = make_uint2(pack_bf16(y0, y1), pack_bf16(y2, y3));
+      if (of) *reinterpret_cast<float4*>(of + ((long long)b * S + r) * ldof + c) = make_float4(y0, y1, y2, y3);
+    }
+  }
+}
+
 }  // namespace ttb
 using namespace ttb;
 
@@ -458,6 +563,31 @@ extern "C" int ttb_groupnorm_apply(const float* x, int B, int S, int C, int grou
   return 0;
 }
 
+// 2 channels per group (gn_stats_pairs_kernel): C / 4 a power of two <= 256, no scale_shift
+static int launch_gn_pairs(const float* x, int B, int S, int C, int groups, const float* gamma, const float* beta,
+                           const float* scale_shift, int do_silu, float* partials, __nv_bfloat16* ob, int ldo,
+                           float* of, int ldof, cudaStream_t st) {
+  const int tpr = C >> 2;
+  if (tpr > 256 || (tpr & (tpr - 1)) || scale_shift || B <= 0 || S <= 0 || (ob && (ldo < C || (ldo & 3))) ||
+      (of && (ldof < C || (ldof & 3)))) {
+    set_error("ttb_groupnorm: 2 channels per group needs C / 4 a power of two <= 256, no scale_shift, S > 0 and "
+              "ldo / ldof >= C, multiples of 4 (C=%d S=%d ldo=%d ldof=%d)", C, S, ldo, ldof);
+    return -1;
+  }
+  const int rows_par = 256 / tpr;
+  int splits = (S + 8 * rows_par - 1) / (8 * rows_par);
+  splits = splits < 1 ? 1 : (splits > TTB_GN_SPLITS ? TTB_GN_SPLITS : splits);
+  const int rows_per_s = (S + splits - 1) / splits;
+  splits = (S + rows_per_s - 1) / rows_per_s;
+  launch_pdl(gn_stats_pairs_kernel, dim3(splits, B), dim3(256), (size_t)0, st, x, S, C, groups, tpr, rows_per_s, partials);
+  TTB_CHECK_LAUNCH("gn_stats_pairs_kernel");
+  const int rows_per_a = 16 * rows_par;
+  launch_pdl(gn_apply_pairs_kernel, dim3((S + rows_per_a - 1) / rows_per_a, B), dim3(256), (size_t)0, st,
+      x, S, C, groups, tpr, rows_per_a, splits, (const float*)partials, gamma, beta, do_silu, ob, ldo, of, ldof, gn_early());
+  TTB_CHECK_LAUNCH("gn_apply_pairs_kernel");
+  return 0;
+}
+
 extern "C" int ttb_groupnorm(const float* x, int B, int S, int C, int groups, const float* gamma, const float* beta,
                              const float* scale_shift, int ss_bstride, const int* ss_row, int ss_row_stride,
                              int do_silu, float* partials, void* out_bf16, int ldo, float* out_f32, int ldof,
@@ -465,6 +595,8 @@ extern "C" int ttb_groupnorm(const float* x, int B, int S, int C, int groups, co
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (C % groups != 0 || (C & 3)) { set_error("ttb_groupnorm: C=%d groups=%d unsupported", C, groups); return -1; }
   const int cpg = C / groups;
+  if (cpg == 2) return launch_gn_pairs(x, B, S, C, groups, gamma, beta, scale_shift, do_silu, partials,
+                                       reinterpret_cast<__nv_bfloat16*>(out_bf16), ldo, out_f32, ldof, st);
   if (cpg % 4 != 0 && (cpg & 3)) { set_error("ttb_groupnorm: channels per group must be a multiple of 4"); return -1; }
   auto is_pow2 = [](int v) { return v > 0 && (v & (v - 1)) == 0; };
   const int cols = C >> 2, lpg = cpg >> 2;

@@ -371,6 +371,32 @@ def synth_wav2vec(cfg="small", seed=0):
     return cfg, sd, vocab
 
 
+def synth_classifier(seed=0):
+    """Seeded `classifier.pth` (AudioMiniEncoderWithClassifierHead of `classify_audio_clip`, api.py:133-145): the
+    reference key layout, 122 tensors. The zero-initialised out_layers.3 and proj_out are drawn like the other convs.
+    The head is drawn at unit gain: the two logits of tone-plus-noise clips then differ by about one, which keeps the
+    softmax away from saturation, where it would hide errors. Not part of synth_all."""
+    g = _Gen(seed * 1000 + 10)
+    sd = {"enc.init.0.weight": g.lin((32, 1, 3), 3), "enc.init.0.bias": g.bias(32)}
+    C, i = 32, 0
+    for _ in range(5):
+        for _ in range(2):
+            p = f"enc.res.{i}."
+            sd[p + "in_layers.0.weight"], sd[p + "in_layers.0.bias"] = g.gamma(C), g.beta(C)
+            sd[p + "in_layers.2.weight"], sd[p + "in_layers.2.bias"] = g.lin((C, C, 5), 5 * C), g.bias(C)
+            sd[p + "out_layers.0.weight"], sd[p + "out_layers.0.bias"] = g.gamma(C), g.beta(C)
+            sd[p + "out_layers.3.weight"], sd[p + "out_layers.3.bias"] = g.lin((C, C, 5), 5 * C, 0.5), g.bias(C)
+            i += 1
+        sd[f"enc.res.{i}.op.weight"], sd[f"enc.res.{i}.op.bias"] = g.lin((2 * C, C, 5), 5 * C), g.bias(2 * C)
+        C, i = 2 * C, i + 1
+    sd["enc.final.0.weight"], sd["enc.final.0.bias"] = g.gamma(C), g.beta(C)
+    sd["enc.final.2.weight"], sd["enc.final.2.bias"] = g.lin((512, C, 1), C), g.bias(512)
+    for a in range(4):
+        _attention_block(sd, g, f"enc.attn.{a}.", 512, 4, False)
+    sd["head.weight"], sd["head.bias"] = g.lin((2, 512), 512), g.bias(2)
+    return sd
+
+
 def synth_all(cfg: ModelConfig, seed=0, suppress_stop=True):
     return {
         "autoregressive": synth_autoregressive(cfg, seed, suppress_stop),
