@@ -34,3 +34,17 @@ def check_sampled_mel(name, mel, ref):
     report("%s rms" % name, rms)
     assert rms < 0.3 and q < 1.5 and mx < 4.0, (name, mx, q, rms)
     return mx, q, rms
+
+
+def rel_live(got, want):
+    """Logit error relative to the scale of the LIVE logits: the synthetic checkpoint pins the start / stop token biases at
+    -1e4 (SURVEY 8d), which would otherwise set the scale and hide a 1e4 x larger error."""
+    live = want.float() > -1e3
+    g, w = got.float()[live], want.float()[live]
+    return (g - w).abs().max().item() / max(w.abs().max().item(), 1e-6)
+
+
+def cuda_sd(sd):
+    """A state dict with every tensor on the current CUDA device (the oracle run on the GPU)."""
+    import torch
+    return {k: (v.cuda() if torch.is_tensor(v) else v) for k, v in sd.items()}

@@ -15,7 +15,7 @@ import os
 import pytest
 import torch
 
-from gpu_util import check_sampled_mel, report
+from gpu_util import check_sampled_mel, cuda_sd, rel_live, report
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -23,18 +23,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 def _rel(a, b):
     return (a.float() - b.float()).abs().max().item() / max(b.float().abs().max().item(), 1e-6)
-
-
-def _rel_live(got, want):
-    """Logit error relative to the scale of the LIVE logits: the synthetic checkpoint pins the start / stop token biases at
-    -1e4 (SURVEY 8d), which would otherwise set the scale and hide a 1e4 x larger error."""
-    live = want.float() > -1e3
-    g, w = got.float()[live], want.float()[live]
-    return (g - w).abs().max().item() / max(w.abs().max().item(), 1e-6)
-
-
-def _cuda_sd(sd):
-    return {k: (v.cuda() if torch.is_tensor(v) else v) for k, v in sd.items()}
 
 
 def _tokens():
@@ -60,10 +48,10 @@ def test_ar_teacher_forced_full_depth_T169_N430(full):
     cond = torch.randn(1, cfg.ar_dim) * 0.5
     codes = torch.randint(0, 8192, (2, 430))
     got = AREngine(sd, cfg).teacher_forced_logits(cond, toks, codes)
-    sdc = _cuda_sd(sd)
+    sdc = cuda_sd(sd)
     with torch.no_grad(), torch.device("cuda"):
         want = ar.teacher_forced_logits(sdc, cfg, cond.cuda(), toks, codes.cuda())
-    r = _rel_live(got, want.to(got.device))
+    r = rel_live(got, want.to(got.device))
     report("prod AR teacher-forced logits T=169 N=430 L=30 (live-logit scale)", r)
     assert r < 0.03
 
@@ -84,10 +72,10 @@ def test_ar_decode_loop_full_depth_prompt174(full):
     tr = []
     codes = AREngine(sd, cfg).generate(cond, toks, B, N, uniforms=u, trace_logits=tr).long()
     seen = torch.stack(tr, 1)
-    sdc = _cuda_sd(sd)
+    sdc = cuda_sd(sd)
     with torch.no_grad(), torch.device("cuda"):
         want = ar.teacher_forced_logits(sdc, cfg, cond.cuda(), toks, codes[:, :-1].cuda())
-    r = _rel_live(seen, want.to(seen.device))
+    r = rel_live(seen, want.to(seen.device))
     report("prod AR decode-loop logits P=174 L=30 (48 steps, live-logit scale)", r)
     assert r < 0.03
 
@@ -103,7 +91,7 @@ def test_clvp_full_depth_L430(full):
     torch.manual_seed(2)
     codes = torch.randint(0, 8192, (2, 430))
     got = CLVPEngine(sd, cfg).scores(toks, codes)
-    sdc = _cuda_sd(sd)
+    sdc = cuda_sd(sd)
     with torch.no_grad(), torch.device("cuda"):
         want = clvp.scores(sdc, cfg, torch.tensor(toks), codes.cuda())
     e = (got - want).abs().max().item()
@@ -126,7 +114,7 @@ def test_denoiser_forward_full_depth_S1872(full):
     x = torch.randn(1, 100, S)
     eng = DiffusionEngine(sd, cfg)
     ce_g = eng.timestep_independent(lat, cond, S)
-    sdc = _cuda_sd(sd)
+    sdc = cuda_sd(sd)
     with torch.no_grad(), torch.device("cuda"):
         ce = od.timestep_independent(sdc, cfg, lat.cuda().unsqueeze(0), cond.cuda().unsqueeze(0), S)
         r = _rel(ce_g.t(), ce[0])
@@ -171,7 +159,7 @@ def test_sampled_mel_200_steps(full):
     mel_g, trace_g = eng.sample(lat, cond, iters, noise0, step_noise, cond_free=True, cond_free_k=2.0, return_trace=True)
     mel_graph = eng.sample(lat, cond, iters, noise0, step_noise, cond_free=True, cond_free_k=2.0, use_graph=True)
     assert (mel_graph - mel_g).abs().max().item() < 1e-3, "graph replay and eager loop disagree"
-    sdc = _cuda_sd(sd)
+    sdc = cuda_sd(sd)
     with torch.no_grad(), torch.device("cuda"):
         ce = od.timestep_independent(sdc, cfg, lat.cuda().unsqueeze(0), cond.cuda().unsqueeze(0), S)
         x_o, trace_o = od.p_sample_loop(sdc, cfg, ce, noise0.cuda().unsqueeze(0), step_noise.cuda().unsqueeze(1), iters,
@@ -203,7 +191,7 @@ def test_vocoder_S1872():
     mel = torch.randn(100, S) * 2 - 5
     z = torch.randn(64, S + 10)
     wav = VocoderEngine(sd, cfg).inference(mel, z)
-    sdc = _cuda_sd(sd)
+    sdc = cuda_sd(sd)
     with torch.no_grad(), torch.device("cuda"):
         want = ov.inference(sdc, mel.cuda().unsqueeze(0), z.cuda().unsqueeze(0))[0, 0]
     e = (wav - want).abs().max().item()
