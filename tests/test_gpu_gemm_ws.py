@@ -4,8 +4,6 @@ of 128x128 tiles) against the one-tile kernel (variant 1) and the SIMT checker (
 Both wgmma kernels add the same k16 products in the same order and finish every 32x32 block with the same epilogue
 code, so variant 7 must reproduce variant 1 bit for bit: outputs and GroupNorm partials. The SIMT checker sums in
 another order; it is held to fp32 accumulation noise relative to the output scale."""
-import os
-
 import pytest
 import torch
 
@@ -105,7 +103,6 @@ def test_ws_against_simt_checker(name):
         assert err <= tol, "%s: max |diff| %.3e > %.3e" % (what, err, tol)
 
 
-@pytest.mark.skipif(os.environ.get("TTB_GEMM_WS") == "0", reason="TTB_GEMM_WS=0 selects the one-tile kernel")
 def test_ws_is_default_for_one_wave():
     """Variant 0 at the diffusion k=3 shape takes the warp-specialised kernel: bit-identical to forcing variant 7."""
     kw = _case("diff_conv_k3")

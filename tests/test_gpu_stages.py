@@ -544,10 +544,9 @@ def test_api_fast_tts_and_stream(which, small, medium):
 
 
 @pytest.mark.gpu
-def test_diffusion_branch_chains_equal_batched(medium):
-    """TTB_DIFF_CHAINS=1: the two CFG branches of a denoiser evaluation as two kernel chains on two streams instead of
-    one batched pass. Every kernel treats the batch items independently, so the model outputs and a sampled mel (6 steps,
-    CUDA graph) must equal the batched run bit for bit (full width, S = 374)."""
+def test_diffusion_sample_repeats_exactly(medium):
+    """Two CUDA-graph samples (6 steps, full width, S = 374) after an eager denoiser evaluation are bit-identical: no
+    kernel of the step sums in a run-dependent order, and the captured graph replays from the rewound state."""
     from tortoise_tts_b200.diffusion_engine import DiffusionEngine
     cfg, sds = medium
     torch.manual_seed(5)
@@ -558,16 +557,9 @@ def test_diffusion_branch_chains_equal_batched(medium):
     x = torch.randn(100, S)
     noise0 = torch.randn(100, S)
     step_noise = torch.randn(6, 100, S)
-    outs = []
-    for chains in (0, 1):
-        eng = DiffusionEngine(sds["diffusion"], cfg)
-        eng.CHAINS = chains
-        ce = eng.timestep_independent(lat, cond, S)
-        c, u = eng.forward_once(x, 1234, ce)
-        assert (eng._ws["branches"] is not None) == bool(chains)
-        mel = eng.sample(lat, cond, 6, noise0, step_noise, cond_free=True, cond_free_k=2.0)
-        mel2 = eng.sample(lat, cond, 6, noise0, step_noise, cond_free=True, cond_free_k=2.0)
-        assert torch.equal(mel, mel2)
-        outs.append((c.cpu(), u.cpu(), mel.cpu()))
-    for a, b in zip(outs[0], outs[1]):
-        assert torch.equal(a, b)
+    eng = DiffusionEngine(sds["diffusion"], cfg)
+    ce = eng.timestep_independent(lat, cond, S)
+    eng.forward_once(x, 1234, ce)
+    mel = eng.sample(lat, cond, 6, noise0, step_noise, cond_free=True, cond_free_k=2.0)
+    mel2 = eng.sample(lat, cond, 6, noise0, step_noise, cond_free=True, cond_free_k=2.0)
+    assert torch.equal(mel, mel2)

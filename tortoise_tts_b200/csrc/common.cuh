@@ -23,27 +23,18 @@ int check_cuda(cudaError_t e, const char* what);
 // ------------------------------------------------------------------ programmatic dependent launch (PDL)
 // Every kernel of the two per-step CUDA graphs starts with pdl_launch_dependents() and calls pdl_wait() before its
 // first access to global memory that an earlier kernel may have written (and before its own first global write).
-// Launched the ordinary way both instructions are no-ops. With TTB_PDL=1 the host launches these kernels with
+// Launched the ordinary way both instructions are no-ops. launch_pdl launches these kernels with
 // cudaLaunchAttributeProgrammaticStreamSerialization: the next kernel's CTAs are scheduled, run their prologue
 // (barrier init, descriptor prefetch) and park in griddepcontrol.wait while the previous kernel drains, which removes
-// the kernel-to-kernel launch gap that dominates the short decode-step kernels. The triggers sit at the kernels' TAILS
-// (GEMM: once all loads of the CTA are issued and its accumulator is complete; LayerNorm: after its loads; others: at
-// exit): a trigger at the top makes the dependent's CTAs resident at once, and they take registers / shared memory
-// away from the kernel still running. On by default; TTB_PDL=0 restores plain launches.
+// the kernel-to-kernel launch gap that dominates the short decode-step kernels. Most triggers sit at the kernels'
+// TAILS (GEMM: once all loads of the CTA are issued and its accumulator is complete; others: at exit): a trigger at
+// the top makes the dependent's CTAs resident at once, and they take registers / shared memory away from the kernel
+// still running. The warp-per-row LayerNorm and the row-wise GroupNorm apply kernels trigger at their start: they
+// need little of either, and the GEMM that follows streams its weight tiles in the meantime (TtbGemmArgs.w_static).
 TTB_DEVINL void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 TTB_DEVINL void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
-inline bool pdl_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("TTB_PDL");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v == 1;
-}
-
-// kernel<<<grid, block, smem, st>>>(args...) with the PDL launch attribute when TTB_PDL=1. Only for kernels that
-// contain pdl_wait().
+// kernel<<<grid, block, smem, st>>>(args...) with the PDL launch attribute. Only for kernels that contain pdl_wait().
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
   cudaLaunchConfig_t cfg = {};
@@ -52,12 +43,10 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
   cudaLaunchAttribute at[1];
-  if (pdl_enabled()) {
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at;
-    cfg.numAttrs = 1;
-  }
+  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  at[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = at;
+  cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 
@@ -196,12 +185,6 @@ TTB_DEVINL void tma_load_3d(void* smem_dst, const CUtensorMap* map, uint64_t* ba
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
-}
-// L2 prefetch of one box of a 3-D tensor map (no shared-memory destination, no barrier)
-TTB_DEVINL void tma_prefetch_l2_3d(const CUtensorMap* map, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.prefetch.tensor.3d.L2.global.tile [%0, {%1, %2, %3}];"
-               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(c2)
-               : "memory");
 }
 
 // ------------------------------------------------------------------ wgmma (Hopper warpgroup MMA)

@@ -218,14 +218,7 @@ flash_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
   pdl_launch_dependents();
 }
 
-static int g_fa_mode = -1;  // 1 = wgmma (default), 0 = SIMT (TTB_ATTN_IMPL=simt)
-
 bool flash_attention_supported(const TtbAttnArgs& a) {
-  if (g_fa_mode < 0) {
-    const char* e = getenv("TTB_ATTN_IMPL");
-    g_fa_mode = (e && strcmp(e, "simt") == 0) ? 0 : 1;
-  }
-  if (!g_fa_mode) return false;
   if (a.kv || a.lse) return true;      // split Q / KV tensors and LSE output exist only in the wgmma kernel
   return a.T >= 64 && (a.ld % 8) == 0;
 }

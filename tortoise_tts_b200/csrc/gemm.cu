@@ -199,27 +199,21 @@ gemm_bf16_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_cons
   }
   __syncthreads();
   // W is a parameter (TtbGemmArgs.w_static): under programmatic dependent launch its tiles do not have to wait for the
-  // kernels before this one. The first STAGES weight tiles go into the pipeline and the rest of this CTA's weight slab
-  // is pulled into L2 BEFORE griddepcontrol.wait; only the activation tiles are requested after it. For the skinny
-  // decode GEMMs (a 64 KB slab per CTA in front of a short main loop) the weights then stream while the previous kernel
-  // (LayerNorm, which triggers its dependents early) is still running.
+  // kernels before this one. The first STAGES weight tiles go into the pipeline BEFORE griddepcontrol.wait; only the
+  // activation tiles are requested after it. For the skinny decode GEMMs (a 64 KB slab per CTA in front of a short
+  // main loop) the weights then stream while the previous kernel (LayerNorm, which triggers its dependents early) is
+  // still running.
   int pre = 0;
   if constexpr (!SPLIT_PRODUCER) {
     if (ep.wpre && warp == PRODUCER_WARP && lane == 0) {
       pre = num_kb < STAGES ? num_kb : STAGES;
-      for (int kbi = 0; kbi < num_kb; ++kbi) {
+      for (int kbi = 0; kbi < pre; ++kbi) {
         const int kb = kb_begin + kbi;
         const int tap = kb / kblocks_per_tap;
         const int kk = (kb - tap * kblocks_per_tap) * BK;
-        if (kbi < pre) {
-          uint8_t* sb = smem + kbi * L::STAGE_BYTES + L::A_BYTES;
-          mbar_arrive_expect_tx(&full_bar[kbi], L::STAGE_BYTES);
-          tma_load_3d(sb, &map_b, &full_bar[kbi], tap * K + kk, n0, 0);
-        } else if (ep.wpre > 1) {
-          tma_prefetch_l2_3d(&map_b, tap * K + kk, n0, 0);
-        } else {
-          break;
-        }
+        uint8_t* sb = smem + kbi * L::STAGE_BYTES + L::A_BYTES;
+        mbar_arrive_expect_tx(&full_bar[kbi], L::STAGE_BYTES);
+        tma_load_3d(sb, &map_b, &full_bar[kbi], tap * K + kk, n0, 0);
       }
     }
   }
@@ -336,7 +330,6 @@ __global__ void gemm_ref_kernel(const __nv_bfloat16* A, long long a_bstride, int
   if (ep.out_bf16) ep.out_bf16[(long long)bz * ep.outb_bstride + (long long)m * ep.ldob + on] = __float2bfloat16(v);
 }
 
-static int g_gemm_impl = -1;  // 0 = wgmma, 1 = SIMT reference (bring-up only; TTB_GEMM_IMPL=ref)
 static unsigned long long* g_gemm_trace = nullptr;   // ttb_debug_gemm_trace
 
 template <int BN, int STAGES, bool SPLIT_PRODUCER = false>
@@ -468,12 +461,9 @@ extern "C" int ttb_gemm(const TtbGemmArgs* gp, void* stream) {
   ep.res_bstride = g.res_bstride; ep.outf_bstride = g.outf_bstride; ep.outb_bstride = g.outb_bstride;
   ep.ldr = g.ldr; ep.ldo = g.ldo; ep.ldob = g.ldob; ep.act = g.act; ep.alpha = g.alpha;
   ep.gn_part = nullptr; ep.gn_groups = g.gn_groups;
-  static int wpre_on = -1;      // TTB_GEMM_WPREFETCH=0: A/B switch for the weight fetch ahead of griddepcontrol.wait
-  // 1 = the first STAGES weight tiles only, 2 = + L2 prefetch of the rest of the CTA's slab
-  if (wpre_on < 0) { const char* e = getenv("TTB_GEMM_WPREFETCH"); wpre_on = e ? atoi(e) : 1; }
-  ep.wpre = g.w_static ? wpre_on : 0;
+  ep.wpre = g.w_static;
   ep.tap_dil = g.tap_dilation > 1 ? g.tap_dilation : 1;
-  if (ep.tap_dil > 1 && (g.cluster > 1 || g.variant == 6 || g.force_ref || g_gemm_impl == 1)) {
+  if (ep.tap_dil > 1 && (g.cluster > 1 || g.variant == 6 || g.force_ref)) {
     set_error("ttb_gemm: tap_dilation is implemented by the one-tile and the persistent kernels only");
     return -1;
   }
@@ -485,19 +475,15 @@ extern "C" int ttb_gemm(const TtbGemmArgs* gp, void* stream) {
     }
     ep.gn_part = reinterpret_cast<float2*>(g.gn_partials + 16);   // scratch layout of norm.cu: 16 floats, then the partials
   }
-  if (g_gemm_impl < 0) {
-    const char* e = getenv("TTB_GEMM_IMPL");
-    g_gemm_impl = (e && strcmp(e, "ref") == 0) ? 1 : 0;
-  }
   if (g.splitk > 1) {
     // split-K writes raw fp32 partials [split, M, ldo] (consumed by ttb_residual_layernorm); no epilogue fusion
     if (g.batch != 1 || g.act != TTB_ACT_NONE || !g.out_f32 || g.out_bf16 || g.bias || g.residual) {
       set_error("ttb_gemm: splitk needs batch=1, no activation/bias/residual and an fp32 partial buffer");
       return -1;
     }
-    if (g_gemm_impl == 1 || g.force_ref) { set_error("ttb_gemm: splitk is not available in the SIMT checker"); return -1; }
+    if (g.force_ref) { set_error("ttb_gemm: splitk is not available in the SIMT checker"); return -1; }
   }
-  if (g_gemm_impl == 1 || g.force_ref) {
+  if (g.force_ref) {
     dim3 block(128), grid((g.N + 127) / 128, g.M, g.batch);
     gemm_ref_kernel<<<grid, block, 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(g.A), g.a_bstride, g.lda, g.rows,
                                             reinterpret_cast<const __nv_bfloat16*>(g.W), g.M, g.N, g.K, g.taps, g.pad, ep);
@@ -523,33 +509,20 @@ extern "C" int ttb_gemm(const TtbGemmArgs* gp, void* stream) {
     if (g.splitk > 1) { set_error("ttb_gemm: variant 7 (warp-specialised 128x256) has no split-K"); return -1; }
     return launch_ws(g, ep, st);
   }
-  static int persist = -1;   // TTB_GEMM_PERSIST=1 sends problems of >= 2 waves to the persistent kernel (A/B comparison)
-  if (persist < 0) { const char* e = getenv("TTB_GEMM_PERSIST"); persist = e ? atoi(e) : 0; }
-  // Off by default: on H100 (80GB HBM3, 700 W) the 128x128 one-tile kernel was faster than this persistent kernel on
-  // every stage that has several tiles per SM (standard preset: CLVP 156 -> 118 ms, diffusion 1061 -> 992 ms).
+  // The persistent 128x128 kernel only on request: on H100 (80GB HBM3, 700 W) the one-tile kernel was faster on every
+  // stage that has several tiles per SM (standard preset: CLVP 156 -> 118 ms, diffusion 1061 -> 992 ms).
   if (g.variant == 2) {
     if (g.tile_n == 32) return launch_persistent<32, 8>(g, ep, st);
     if (g.tile_n == 64) return launch_persistent<64, 6>(g, ep, st);
     return launch_persistent<128, 4>(g, ep, st);
   }
-  const int use_persist = (g.variant == 1) ? 0 : persist;
-  if (use_persist && g.tile_n == 0 && tiles128 >= 2 * num_sms()) return launch_persistent<128, 4>(g, ep, st);
-  if (use_persist == 2) {        // TTB_GEMM_PERSIST=2: force the persistent kernels everywhere (experiments)
-    if (g.tile_n == 32) return launch_persistent<32, 8>(g, ep, st);
-    if (g.tile_n == 64 || (g.tile_n == 0 && tiles128 < num_sms())) return launch_persistent<64, 6>(g, ep, st);
-    if (g.tile_n != 256) return launch_persistent<128, 4>(g, ep, st);
-  }
   // Default for problems of at least one wave of 128x128 tiles: the persistent warp-specialised 128x256 kernel
-  // (gemm_ws.cuh). TTB_GEMM_WS=0 restores the one-tile 128x128 kernel (A/B runs).
-  static int ws = -1;
-  if (ws < 0) { const char* e = getenv("TTB_GEMM_WS"); ws = e ? atoi(e) : 1; }
-  if (ws && g.tile_n == 0 && g.variant == 0 && g.splitk <= 1 && tiles128 >= num_sms()) return launch_ws(g, ep, st);
+  // (gemm_ws.cuh). variant 1 keeps the one-tile 128x128 kernel.
+  if (g.tile_n == 0 && g.variant == 0 && g.splitk <= 1 && tiles128 >= num_sms()) return launch_ws(g, ep, st);
   if (g.tile_n == 32) {
     // the skinny decode GEMMs are latency-bound (k-block time = TMA round trip / stages): 5 stages still allow two
-    // CTAs per SM (2 x 101 KB of the 227 KB). TTB_GEMM_T32_STAGES=4 restores the 4-stage kernel for A/B runs; variant 3 forces 5.
-    static int t32 = -1;
-    if (t32 < 0) { const char* e = getenv("TTB_GEMM_T32_STAGES"); t32 = e ? atoi(e) : 5; }
-    return (g.variant == 3 || (g.variant != 4 && t32 == 5)) ? launch_tc<32, 5>(g, ep, st) : launch_tc<32, 4>(g, ep, st);
+    // CTAs per SM (2 x 101 KB of the 227 KB). variant 4 selects the 4-stage kernel.
+    return g.variant == 4 ? launch_tc<32, 4>(g, ep, st) : launch_tc<32, 5>(g, ep, st);
   }
   // 64-wide tiles, 8 stages, one CTA per SM (variant 3): for skinny problems whose 64-wide grid fits one wave, the deep
   // pipeline keeps ~190 KB in flight per SM

@@ -57,22 +57,16 @@ gemm_bf16_ws_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_cons
   }
   __syncthreads();
   // TtbGemmArgs.w_static (see the one-tile kernel): the weight halves of the first tile's first stages are requested
-  // before griddepcontrol.wait (with wpre > 1 the rest of that tile's weight slab is pulled into L2 as well).
+  // before griddepcontrol.wait.
   int pre = 0;
   if (ep.wpre && threadIdx.x == 0) {
     const int n0 = ((blockIdx.x / m_tiles) % n_tiles) * WS_BN;
     pre = num_kb < WS_STAGES ? num_kb : WS_STAGES;
-    for (int kb = 0; kb < num_kb; ++kb) {
+    for (int kb = 0; kb < pre; ++kb) {
       const int tap = kb / kblocks_per_tap;
       const int kk = (kb - tap * kblocks_per_tap) * BK;
-      if (kb < pre) {
-        mbar_arrive_expect_tx(&full_bar[kb], L::STAGE_BYTES);
-        tma_load_3d(smem + kb * L::STAGE_BYTES + L::A_BYTES, &map_b, &full_bar[kb], tap * K + kk, n0, 0);
-      } else if (ep.wpre > 1) {
-        tma_prefetch_l2_3d(&map_b, tap * K + kk, n0, 0);
-      } else {
-        break;
-      }
+      mbar_arrive_expect_tx(&full_bar[kb], L::STAGE_BYTES);
+      tma_load_3d(smem + kb * L::STAGE_BYTES + L::A_BYTES, &map_b, &full_bar[kb], tap * K + kk, n0, 0);
     }
   }
   pdl_wait();                    // activations, residual and outputs belong to earlier kernels until here

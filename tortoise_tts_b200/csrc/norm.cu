@@ -82,12 +82,12 @@ __global__ void __launch_bounds__(64)
 layernorm_warp_kernel(const float* x, int M, int D, const float* __restrict__ g1, const float* __restrict__ b1,
                       const float* __restrict__ g2, const float* __restrict__ b2, __nv_bfloat16* __restrict__ ob,
                       float* __restrict__ of, float* xw, const float* __restrict__ partials, int nsplit,
-                      long long split_stride, const float* __restrict__ rbias, int early) {
-  // `early`: let the next kernel's CTAs start NOW (TTB_LN_EARLY, default on). In the decode step that kernel is a
-  // skinny GEMM with TtbGemmArgs.w_static: it runs its prologue and streams its weight tiles while this kernel works,
-  // and still waits (griddepcontrol.wait) for this grid to finish before it touches the normalised rows. This kernel
-  // needs no shared memory and few registers, so the early CTAs take nothing away from it.
-  if (early) pdl_launch_dependents();
+                      long long split_stride, const float* __restrict__ rbias) {
+  // Let the next kernel's CTAs start at once. In the decode step that kernel is a skinny GEMM with
+  // TtbGemmArgs.w_static: it runs its prologue and streams its weight tiles while this kernel works, and still waits
+  // (griddepcontrol.wait) for this grid to finish before it touches the normalised rows. This kernel needs no shared
+  // memory and few registers, so the early CTAs take nothing away from it.
+  pdl_launch_dependents();
   pdl_wait();
   const int lane = threadIdx.x & 31;
   const long long row = (long long)blockIdx.x * 2 + (threadIdx.x >> 5);
@@ -115,7 +115,6 @@ layernorm_warp_kernel(const float* x, int M, int D, const float* __restrict__ g1
       *reinterpret_cast<float4*>(xw + row * D + (i * 32 + lane) * 4) = v[i];
     }
   }
-  if (!early) pdl_launch_dependents();        // tail trigger: every load of this row is done
 #pragma unroll
   for (int pass = 0; pass < 2; ++pass) {
     const float* gg = pass == 0 ? g1 : g2;
@@ -312,8 +311,8 @@ __global__ void __launch_bounds__(256)
 gn_apply_rows_kernel(const float* __restrict__ x, int S, int C, int groups, int cpg, int tpr, int rows_per, int splits,
                      const float* __restrict__ scratch, const float* __restrict__ gamma, const float* __restrict__ beta,
                      const float* __restrict__ ss, int ss_bstride, const int* __restrict__ ss_row, int ss_row_stride,
-                     int do_silu, __nv_bfloat16* __restrict__ ob, int ldo, float* __restrict__ of, int ldof, int early) {
-  if (early) pdl_launch_dependents();   // TTB_GN_EARLY (default on): as layernorm_warp_kernel, for the GEMM that follows
+                     int do_silu, __nv_bfloat16* __restrict__ ob, int ldo, float* __restrict__ of, int ldof) {
+  pdl_launch_dependents();   // as layernorm_warp_kernel, for the GEMM that follows
   pdl_wait();
   const int b = blockIdx.y;
   const int rows_par = 256 / tpr;
@@ -422,8 +421,8 @@ gn_stats_pairs_kernel(const float* __restrict__ x, int S, int C, int groups, int
 __global__ void __launch_bounds__(256)
 gn_apply_pairs_kernel(const float* __restrict__ x, int S, int C, int groups, int tpr, int rows_per, int splits,
                       const float* __restrict__ scratch, const float* __restrict__ gamma, const float* __restrict__ beta,
-                      int do_silu, __nv_bfloat16* __restrict__ ob, int ldo, float* __restrict__ of, int ldof, int early) {
-  if (early) pdl_launch_dependents();
+                      int do_silu, __nv_bfloat16* __restrict__ ob, int ldo, float* __restrict__ of, int ldof) {
+  pdl_launch_dependents();
   pdl_wait();
   const int b = blockIdx.y;
   const int rows_par = 256 / tpr;
@@ -479,27 +478,17 @@ gn_apply_pairs_kernel(const float* __restrict__ x, int S, int C, int groups, int
 using namespace ttb;
 
 // warp-per-row LayerNorm when the row is NV x 128 floats and everything is 16-byte aligned; false = not applicable
-static int gn_early() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("TTB_GN_EARLY"); v = (e && e[0] == '0') ? 0 : 1; }     // default on
-  return v;
-}
-
 static bool launch_ln_warp(const float* x, int M, int D, const float* g1, const float* b1, const float* g2, const float* b2,
                            __nv_bfloat16* ob, float* of, float* xw, const float* partials, int nsplit,
                            long long split_stride, const float* rbias, cudaStream_t st) {
-  const char* impl = getenv("TTB_LN_IMPL");          // "block" forces the block-per-row kernel (A/B timing)
-  if (impl && impl[0] == 'b') return false;
   if (D % 128 != 0 || D > 1024 || (split_stride & 3)) return false;
   const void* ptrs[] = {x, g1, b1, g2, b2, ob, of, xw, partials, rbias};
   for (const void* p : ptrs)
     if (p && (reinterpret_cast<uintptr_t>(p) & 15)) return false;
   const dim3 grid((M + 1) / 2);
-  static int early = -1;
-  if (early < 0) { const char* e = getenv("TTB_LN_EARLY"); early = (e && e[0] == '0') ? 0 : 1; }
 #define TTB_LN_CASE(NV)                                                                                              \
   case NV: launch_pdl(layernorm_warp_kernel<NV>, grid, dim3(64), (size_t)0, st, x, M, D, g1, b1, g2, b2, ob, of, xw,  \
-                      partials, nsplit, split_stride, rbias, early); break;
+                      partials, nsplit, split_stride, rbias); break;
   switch (D / 128) {
     TTB_LN_CASE(1) TTB_LN_CASE(2) TTB_LN_CASE(3) TTB_LN_CASE(4) TTB_LN_CASE(5) TTB_LN_CASE(6) TTB_LN_CASE(7) TTB_LN_CASE(8)
     default: return false;
@@ -558,7 +547,7 @@ extern "C" int ttb_groupnorm_apply(const float* x, int B, int S, int C, int grou
   const int tpr = C >> 2, rows_par = 256 / tpr, rows_per_a = 16 * rows_par;
   launch_pdl(gn_apply_rows_kernel, dim3((S + rows_per_a - 1) / rows_per_a, B), dim3(256), (size_t)0, st,
       x, S, C, groups, 32, tpr, rows_per_a, splits, partials, gamma, beta, scale_shift, ss_bstride, ss_row, ss_row_stride,
-      do_silu, reinterpret_cast<__nv_bfloat16*>(out_bf16), ldo, out_f32, ldof, gn_early());
+      do_silu, reinterpret_cast<__nv_bfloat16*>(out_bf16), ldo, out_f32, ldof);
   TTB_CHECK_LAUNCH("gn_apply_rows_kernel");
   return 0;
 }
@@ -583,7 +572,7 @@ static int launch_gn_pairs(const float* x, int B, int S, int C, int groups, cons
   TTB_CHECK_LAUNCH("gn_stats_pairs_kernel");
   const int rows_per_a = 16 * rows_par;
   launch_pdl(gn_apply_pairs_kernel, dim3((S + rows_per_a - 1) / rows_per_a, B), dim3(256), (size_t)0, st,
-      x, S, C, groups, tpr, rows_per_a, splits, (const float*)partials, gamma, beta, do_silu, ob, ldo, of, ldof, gn_early());
+      x, S, C, groups, tpr, rows_per_a, splits, (const float*)partials, gamma, beta, do_silu, ob, ldo, of, ldof);
   TTB_CHECK_LAUNCH("gn_apply_pairs_kernel");
   return 0;
 }
@@ -600,9 +589,7 @@ extern "C" int ttb_groupnorm(const float* x, int B, int S, int C, int groups, co
   if (cpg % 4 != 0 && (cpg & 3)) { set_error("ttb_groupnorm: channels per group must be a multiple of 4"); return -1; }
   auto is_pow2 = [](int v) { return v > 0 && (v & (v - 1)) == 0; };
   const int cols = C >> 2, lpg = cpg >> 2;
-  const char* impl = getenv("TTB_GN_IMPL");       // "group" forces the generic group-wise kernels (A/B timing)
-  const bool force_group = impl && impl[0] == 'g';
-  if (!force_group && (cpg & 3) == 0 && is_pow2(cols) && cols <= 256 && is_pow2(lpg) && lpg <= 32 && groups <= 256 && S > 0) {
+  if ((cpg & 3) == 0 && is_pow2(cols) && cols <= 256 && is_pow2(lpg) && lpg <= 32 && groups <= 256 && S > 0) {
     // row-wise path (see gn_stats_rows_kernel)
     const int tpr = cols, rows_par = 256 / tpr;
     int splits = (S + 8 * rows_par - 1) / (8 * rows_par);
@@ -614,7 +601,7 @@ extern "C" int ttb_groupnorm(const float* x, int B, int S, int C, int groups, co
     const int rows_per_a = 16 * rows_par;     // two batches of 8 loads per thread; amortises the per-block stats fold
     launch_pdl(gn_apply_rows_kernel, dim3((S + rows_per_a - 1) / rows_per_a, B), dim3(256), (size_t)0, st,
         x, S, C, groups, cpg, tpr, rows_per_a, splits, (const float*)partials, gamma, beta, scale_shift, ss_bstride, ss_row, ss_row_stride,
-        do_silu, reinterpret_cast<__nv_bfloat16*>(out_bf16), ldo, out_f32, ldof, gn_early());
+        do_silu, reinterpret_cast<__nv_bfloat16*>(out_bf16), ldo, out_f32, ldof);
     TTB_CHECK_LAUNCH("gn_apply_rows_kernel");
     return 0;
   }

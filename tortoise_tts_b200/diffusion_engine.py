@@ -158,17 +158,6 @@ class DiffusionEngine:
         self.b_outc = _f(sd["out.2.bias"], dev)
         self.res_all = [r for r, _ in self.integ] + [r for r, _ in self.layers] + self.tail
         self._ws = None
-        # TMA-multicast clusters along N for the C x C convs (TTB_DIFF_CLUSTER=0 disables); needs C/128 tiles % CL == 0
-        import os
-        cl = int(os.environ.get("TTB_DIFF_CLUSTER", "0"))
-        self.CL = cl if (cl in (2, 4) and (C // 128) % cl == 0) else 0
-        # GroupNorm statistics taken in the epilogue of the producing GEMM (TTB_GN_FUSED=0: separate statistics pass)
-        self.GN_FUSED = int(os.environ.get("TTB_GN_FUSED", "1"))
-        # the two CFG branches as two kernel chains on two streams instead of one batched pass (see _forward)
-        self.CHAINS = int(os.environ.get("TTB_DIFF_CHAINS", "0"))
-        # the C x C GEMMs of a step put their first weight tiles into the pipeline ahead of griddepcontrol.wait
-        # (TtbGemmArgs.w_static; the GroupNorm in front of them releases its dependents early); TTB_DIFF_WSTATIC=0 = off
-        self.WS = bool(int(os.environ.get("TTB_DIFF_WSTATIC", "1")))
 
     # ------------------------------------------------------------------ building blocks on [B, S, C] fp32 (in place)
     def _gn(self, x, B, S, g, b, ws, silu=False, ss=None, ss_row=None, out=None, ready=False):
@@ -180,8 +169,9 @@ class DiffusionEngine:
 
     def _gnp(self, S, ws):
         """kwargs that make a C-wide GEMM leave the GroupNorm statistics of its output for the GroupNorm that follows
-        (TtbGemmArgs.gn_partials): 32 channels per group and at most TTB_GROUPNORM_SPLITS row blocks of 32."""
-        if self.GN_FUSED and self.C == 32 * self.groups and (S + 31) // 32 <= 128:
+        (TtbGemmArgs.gn_partials): 32 channels per group and at most TTB_GROUPNORM_SPLITS row blocks of 32. Otherwise
+        the GroupNorm takes its statistics in a separate pass."""
+        if self.C == 32 * self.groups and (S + 31) // 32 <= 128:
             return dict(gn_partials=ws["partials"], gn_groups=self.groups)
         return {}
 
@@ -190,13 +180,15 @@ class DiffusionEngine:
         C, H = self.C, self.H
         gp = self._gnp(S, ws)
         self._gn(x, B, S, aw.gn_g, aw.gn_b, ws, ready=ready)
+        # w_static: the C-wide GEMMs of a step put their first weight tiles into the pipeline ahead of
+        # griddepcontrol.wait (the GroupNorm in front of them releases its dependents at its start)
         lib.gemm(ws["a"], aw.wqkv, M=S, N=3 * C, K=C, bias=aw.bqkv, out_bf16=ws["qkv"], batch=B, a_bstride=S * C,
-                 outb_bstride=S * 3 * C, cluster=self.CL, w_static=self.WS)
+                 outb_bstride=S * 3 * C, w_static=True)
         # T5 buckets saturate at max_distance = 64 (xtransformers.py:166-174): |j - i| >= 64 -> constant bias per side
         lib.attention(ws["qkv"], ws["o"], nseq=B, T=S, H=H, ld=3 * C, ldo=C, k_off=C, v_off=2 * C, scale=0.125,
                       bias=aw.table(S), bias_sat=64)
         lib.gemm(ws["o"], aw.wproj, M=S, N=C, K=C, bias=aw.bproj, residual=x, out_f32=x, batch=B, a_bstride=S * C,
-                 res_bstride=S * C, outf_bstride=S * C, cluster=self.CL, w_static=self.WS, **gp)
+                 res_bstride=S * C, outf_bstride=S * C, w_static=True, **gp)
         return bool(gp)
 
     def _res_block(self, rw, ss, x, B, S, ws, ss_row=None, ready=False):
@@ -205,10 +197,10 @@ class DiffusionEngine:
         gp = self._gnp(S, ws)
         self._gn(x, B, S, rw.in_g, rw.in_b, ws, silu=True, ready=ready)
         lib.gemm(ws["a"], rw.w_in, M=S, N=C, K=C, bias=rw.b_in, out_f32=ws["h"], batch=B, a_bstride=S * C,
-                 outf_bstride=S * C, cluster=self.CL, w_static=self.WS, **gp)
+                 outf_bstride=S * C, w_static=True, **gp)
         self._gn(ws["h"], B, S, rw.out_g, rw.out_b, ws, silu=True, ss=ss, ss_row=ss_row, ready=bool(gp))
         lib.gemm(ws["a"], rw.w_out, M=S, N=C, K=C, taps=3, pad=1, bias=rw.b_out, residual=x, out_f32=x, batch=B,
-                 a_bstride=S * C, res_bstride=S * C, outf_bstride=S * C, cluster=self.CL, w_static=self.WS, **gp)
+                 a_bstride=S * C, res_bstride=S * C, outf_bstride=S * C, w_static=True, **gp)
         return bool(gp)
 
     def _alloc(self, B, S):
@@ -242,24 +234,9 @@ class DiffusionEngine:
 
     # ------------------------------------------------------------------ one denoiser evaluation (both CFG branches)
     def _forward(self, st):
-        """Both CFG branches of one denoiser evaluation. Default: ONE batched pass (B = 2 in every launch). With
-        TTB_DIFF_CHAINS=1 the conditional and the unconditional branch run as two independent kernel chains on two
-        streams (forked / joined with events, still one capturable unit): the flash-attention kernel keeps the tensor
-        pipe ~17 % busy (it is bound by its softmax chain), so the other branch's GEMMs can use the rest of the SM."""
-        br = st.get("branches")
-        if not br:
-            return self._forward_one(st)
-        cur = torch.cuda.current_stream()
-        side = st["side"]
-        side.wait_stream(cur)
-        self._forward_one(br[0])
-        with torch.cuda.stream(side):
-            self._forward_one(br[1])
-        cur.wait_stream(side)
-
-    def _forward_one(self, st):
         """DiffusionTts.forward (diffusion_decoder.py:262-322) for batch [cond, uncond] (or one of them) at the timestep
-        selected by the device-side call counter. Writes st['mo_local'] [B, S, cout]."""
+        selected by the device-side call counter, both CFG branches batched in every launch. Writes st['mo_local']
+        [B, S, cout]."""
         C, B, S, ws = self.C, st["B"], st["S"], st["ws"]
         xce = st["xce"]
         xce.copy_(st["code_emb_init"])
@@ -344,14 +321,6 @@ class DiffusionEngine:
         st["ss_all"] = torch.empty(len(self.res_all), iters, 2 * C, dtype=torch.float32, device=dev)
         st["graph"] = None
         st["xch"] = None
-        st["branches"] = None
-        if B == 2 and self.CHAINS and dev.type == "cuda":
-            # per-branch views of the batched buffers + a workspace of its own for each branch
-            st["branches"] = [dict(B=1, S=S, ws=self._alloc(1, S), xce=st["xce"][b:b + 1],
-                                   code_emb_init=st["code_emb_init"][b:b + 1], cat=st["cat"][b:b + 1], xm=st["xm"][b:b + 1],
-                                   mo_local=st["model_out"][b:b + 1], x_bf=st["x_bf"], ss_all=st["ss_all"],
-                                   counter=st["counter"]) for b in range(2)]
-            st["side"] = torch.cuda.Stream(device=dev)
         if pair is not None and st["model_out"].is_cuda:
             from . import parallel
             xch = parallel.PairExchange(pair[0], pair[1], S * self.cout, dev)
