@@ -213,6 +213,14 @@ typedef struct TtbArStepArgs {
   int attn_compact;                        /* 1: the attention-only launch (debug_phase_mask = 4, one layer) runs in 8-warp CTAs
                                               whose shared memory is sized to the prompt (~118 KB at P = 174), so that CTAs of
                                               another stream fit beside them (two decode chains); same results */
+  /* Prompt groups (several utterances in one batch): groups > 0 (at most 16) replaces prefix_kv / P. Rows
+   * [group_begin[g], group_begin[g + 1]) attend to the prefix group_prefix_kv[g] of group_P[g] positions (<= 352), laid
+   * out [L][H][P_g][2][64] as ttb_ar_step_store_prefix writes it; group_begin[0] = 0, group_begin[groups] = B, every
+   * group non-empty. HOST arrays, read by every call that takes these args. groups = 0: every row shares prefix_kv. */
+  int groups;
+  const int* group_begin;                  /* [groups + 1] */
+  const int* group_P;                      /* [groups] */
+  const void* const* group_prefix_kv;      /* [groups] device pointers */
 } TtbArStepArgs;
 int ttb_ar_step_workspace(const TtbArStepArgs* args, long long* part_floats, long long* table_bytes, long long* sync_bytes);
 int ttb_ar_step_setup(const TtbArStepArgs* args, void* stream);      /* synchronous; once per (weights, workspace, B) */

@@ -369,12 +369,16 @@ class TextToSpeech:
         random.seed(seed)
         return seed
 
-    def tts_with_preset(self, text, preset="fast", **kwargs):
+    @staticmethod
+    def _preset_settings(preset, kwargs):
         settings = {"temperature": .8, "length_penalty": 1.0, "repetition_penalty": 2.0, "top_p": .8,
                     "cond_free_k": 2.0, "diffusion_temperature": 1.0}
         settings.update(PRESETS[preset])
         settings.update(kwargs)
-        return self.tts(text, **settings)
+        return settings
+
+    def tts_with_preset(self, text, preset="fast", **kwargs):
+        return self.tts(text, **self._preset_settings(preset, kwargs))
 
     def tts_long(self, text, preset="standard", shard_utterances=True, text_tokens_list=None, **kwargs):
         """≙ the loop of the reference's `read.py:44-85` for one voice: split the text (`'|'` forces the split points,
@@ -412,6 +416,86 @@ class TextToSpeech:
             wavs = [parts[u] for u in range(len(texts))]
         return torch.cat([w.reshape(1, -1).cpu() for w in wavs], dim=-1)
 
+    def tts_batch(self, texts, preset="standard", text_tokens_list=None, **kwargs):
+        """Several utterances in one call: entry u of the returned list is what
+        `tts_with_preset(texts[u], preset=preset, **kwargs)` returns ([1, 1, S] for k = 1, else a list of k), with the
+        conditioning computed once and ONE seed for every utterance (as tts_long). The utterances' candidates are decoded
+        together: consecutive utterances are packed into decode batches of at most 256 candidates and 16 prompts
+        (ar_engine.plan_batches), each utterance attending to its own prompt, so a small preset does not pay a whole
+        decode step per utterance. An utterance with more than 256 candidates or a prompt longer than 352 positions is
+        decoded alone, as tts() decodes it. Ranking, diffusion, vocoder and redaction then run per utterance as in tts().
+        `text_tokens_list` (one id list per text) bypasses the tokenizer. On several ranks the utterances are spread as
+        tts_long(shard_utterances=True) spreads its chunks (k must be 1); every rank batches its share."""
+        texts = list(texts)
+        if not texts:
+            raise ValueError("tts_batch needs at least one text")
+        if text_tokens_list is not None and len(text_tokens_list) != len(texts):
+            raise ValueError("text_tokens_list has %d entries for %d texts" % (len(text_tokens_list), len(texts)))
+        return self._tts_batch(texts, text_tokens_list, **self._preset_settings(preset, kwargs))
+
+    def _tts_batch(self, texts, text_tokens_list, voice_samples=None, conditioning_latents=None, k=1, verbose=True,
+                   use_deterministic_seed=None, num_autoregressive_samples=512, temperature=.8, length_penalty=1,
+                   repetition_penalty=2.0, top_p=.8, max_mel_tokens=500, cvvp_amount=.0, diffusion_iterations=100,
+                   cond_free=True, cond_free_k=2, diffusion_temperature=1.0, top_k=50, typical_sampling=False,
+                   typical_mass=.9, **hf_generate_kwargs):
+        from .text import utterance_plan
+        from .ar_engine import plan_batches
+        if hf_generate_kwargs:
+            raise TypeError(f"unsupported generate kwargs: {sorted(hf_generate_kwargs)}")
+        rank, ws = parallel.world()
+        if ws > 1 and k != 1:
+            raise NotImplementedError("tts_batch on several ranks renders one waveform per text: k must be 1")
+        typical = _typical_mass(typical_sampling, typical_mass)
+        seed = self.deterministic_state(seed=use_deterministic_seed)
+        auto_cond, diff_cond, auto_conds, _ = self._conditioning(voice_samples, conditioning_latents)
+        plan = utterance_plan(len(texts), ws)
+        mine = [u for u in range(len(texts)) if plan[u] == rank]
+        dev = self.device
+        B, Nmax = int(num_autoregressive_samples), int(max_mel_tokens)
+        ar = self.autoregressive
+        dec = dict(temperature=temperature, top_k=top_k, top_p=top_p, repetition_penalty=repetition_penalty,
+                   pos_mode="ref_kv_quirk" if self.kv_cache else "train_consistent", typical_mass=typical)
+        parts, sums = {}, {}
+        t_ar = 0.0
+        ends = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+        ends[0].record()
+        with parallel.single_rank(), torch.no_grad():
+            toks = {u: self._text_ids(texts[u], None if text_tokens_list is None else text_tokens_list[u]) for u in mine}
+            # the uniforms table tts() draws: the same seed, so the same table for every utterance
+            g = torch.Generator(device=dev)
+            g.manual_seed(seed)
+            uniforms = torch.rand(B, Nmax, generator=g, device=dev)
+            # the grouped step needs the one-kernel step; with the per-op step forced every utterance decodes alone
+            max_groups = 1 if ar.MODE == "perop" else lib.AR_STEP_MAX_GROUPS
+            for batch in plan_batches([(B, len(toks[mine[i]]) + 4) for i in range(len(mine))], max_groups=max_groups):
+                us = [mine[i] for i in batch]
+                ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+                ev[0].record()
+                if len(us) == 1:
+                    codes = [ar.generate(auto_cond, toks[us[0]], B, Nmax, uniforms=uniforms, **dec)]
+                else:
+                    codes = ar.generate_grouped(auto_cond, [toks[u] for u in us], [B] * len(us), Nmax,
+                                                uniforms_list=[uniforms] * len(us), **dec)
+                ev[1].record()
+                for u, c in zip(us, codes):
+                    e = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
+                    res, t = self._render(texts[u], toks[u], c, B, k, seed, auto_cond, diff_cond, auto_conds,
+                                          cvvp_amount, diffusion_iterations, cond_free, cond_free_k,
+                                          diffusion_temperature, e)
+                    parts[u] = res if len(res) > 1 else res[0]
+                    t["clvp_ms"] = e[0].elapsed_time(e[1])
+                    for key, v in t.items():
+                        sums[key] = sums.get(key, 0.0) + v
+                t_ar += ev[0].elapsed_time(ev[1])
+        ends[1].record()
+        ends[1].synchronize()
+        # ar_ms: the decode batches (the grouped AR stage); the other stages summed over this rank's utterances
+        self.last_timings = {"ar_ms": t_ar, **sums, "device_total_ms": ends[0].elapsed_time(ends[1])}
+        if ws == 1:
+            return [parts[u] for u in range(len(texts))]
+        wavs = parallel.exchange_utterances({u: w.reshape(-1) for u, w in parts.items()}, plan, dev)
+        return [w.reshape(1, 1, -1).cpu() for w in wavs]
+
     def tts(self, text, voice_samples=None, conditioning_latents=None, k=1, verbose=True, use_deterministic_seed=None,
             return_deterministic_state=False, num_autoregressive_samples=512, temperature=.8, length_penalty=1,
             repetition_penalty=2.0, top_p=.8, max_mel_tokens=500, cvvp_amount=.0, diffusion_iterations=100,
@@ -424,22 +508,9 @@ class TextToSpeech:
             raise TypeError(f"unsupported generate kwargs: {sorted(hf_generate_kwargs)}")
         typical = _typical_mass(typical_sampling, typical_mass)
         seed = self.deterministic_state(seed=use_deterministic_seed)
-        # api.py:395-401 (after the seeding, so that the random crop / random voice follow use_deterministic_seed)
-        auto_conds = None                 # the conditioning MELs: only known when the clips themselves are given
-        if voice_samples is not None:
-            auto_conditioning, diffusion_conditioning, auto_conds, _ = self.get_conditioning_latents(voice_samples,
-                                                                                                   return_mels=True)
-            conditioning_latents = (auto_conditioning, diffusion_conditioning)
-        elif conditioning_latents is None:
-            conditioning_latents = self.get_random_conditioning_latents()
+        auto_cond, diff_cond, auto_conds, conditioning_latents = self._conditioning(voice_samples, conditioning_latents)
+        toks = self._text_ids(text, text_tokens)
         dev = self.device
-        if text_tokens is None:
-            text_tokens = self.tokenizer.encode(text)
-        toks = [int(t) for t in text_tokens] + [0]            # F.pad(text_tokens, (0, 1)) (api.py:391)
-        assert len(toks) < 400, "Too much text provided. Break the text up into separate segments and re-try inference."
-        auto_cond, diff_cond = conditioning_latents
-        auto_cond = auto_cond.to(dev).float().reshape(-1)
-        diff_cond = diff_cond.to(dev).float().reshape(-1)
         rank, ws = parallel.world()
         B = int(num_autoregressive_samples)
         lo, hi = parallel.shard_range(B, rank, ws)
@@ -456,10 +527,51 @@ class TextToSpeech:
                                                  repetition_penalty=repetition_penalty,
                                                  pos_mode="ref_kv_quirk" if self.kv_cache else "train_consistent",
                                                  typical_mass=typical)
+            res, t = self._render(text, toks, codes, B, k, seed, auto_cond, diff_cond, auto_conds, cvvp_amount,
+                                  diffusion_iterations, cond_free, cond_free_k, diffusion_temperature, ev[1:4])
+            self.last_timings = {"ar_ms": ev[0].elapsed_time(ev[1]), "clvp_ms": ev[1].elapsed_time(ev[2]), **t,
+                                 "device_total_ms": ev[0].elapsed_time(ev[3])}
+        out = res if len(res) > 1 else res[0]
+        if return_deterministic_state:
+            return out, (seed, text, voice_samples, conditioning_latents)
+        return out
+
+    def _conditioning(self, voice_samples, conditioning_latents):
+        """api.py:395-401 (after the seeding, so that the random crop / random voice follow use_deterministic_seed):
+        -> (auto latent [D], diffusion latent [2C] on the device, the conditioning MELs or None, the latent pair). The
+        conditioning MELs are only known when the clips themselves are given."""
+        auto_conds = None
+        if voice_samples is not None:
+            auto_conditioning, diffusion_conditioning, auto_conds, _ = self.get_conditioning_latents(voice_samples,
+                                                                                                   return_mels=True)
+            conditioning_latents = (auto_conditioning, diffusion_conditioning)
+        elif conditioning_latents is None:
+            conditioning_latents = self.get_random_conditioning_latents()
+        auto_cond, diff_cond = conditioning_latents
+        dev = self.device
+        return (auto_cond.to(dev).float().reshape(-1), diff_cond.to(dev).float().reshape(-1), auto_conds,
+                conditioning_latents)
+
+    def _text_ids(self, text, text_tokens):
+        if text_tokens is None:
+            text_tokens = self.tokenizer.encode(text)
+        toks = [int(t) for t in text_tokens] + [0]            # F.pad(text_tokens, (0, 1)) (api.py:391)
+        assert len(toks) < 400, "Too much text provided. Break the text up into separate segments and re-try inference."
+        return toks
+
+    def _render(self, text, toks, codes, B, k, seed, auto_cond, diff_cond, auto_conds, cvvp_amount, diffusion_iterations,
+                cond_free, cond_free_k, diffusion_temperature, ev):
+        """What tts() does after the decode, for one utterance: fix the codes of this rank's candidates, rank all B
+        candidates (CLVP / CVVP, top-k), then latents, calm-token trim, diffusion, vocoder and redaction of the k best.
+        Records ev[0] after the fix, ev[1] after the ranking, ev[2] after the rendering. Returns (list of k waveforms
+        [1, 1, S] on the CPU, {stage: device ms} of the rendering stages)."""
+        dev = self.device
+        rank, ws = parallel.world()
+        with torch.no_grad():
             nb, L = codes.shape
             trim = torch.empty(nb, dtype=torch.int32, device=dev)
             lib.ar_fix_codes(codes, nb, L, self.cfg.stop_mel_token, trim)
-            ev[1].record()
+            ev[0].record()
             # api.py:450-472: CLVP, CVVP (needs the conditioning mels, i.e. voice_samples) or their blend. cvvp_amount = 1
             # without voice_samples leaves `clvp_out` undefined in the reference; CLVP alone is used here.
             use_cvvp = cvvp_amount > 0 and auto_conds is not None
@@ -477,7 +589,7 @@ class TextToSpeech:
             if self.debug_capture:      # parity hook (tests): the intermediate results of the stages of this call
                 self.last_debug = {"seed": seed, "codes": codes.clone(), "scores": scores.clone(), "best": best.clone(),
                                    "latents": {}, "mel": {}, "noise": {}}
-            ev[2].record()
+            ev[1].record()
             # rendering plan: candidate j -> owner rank (+ the rank pair sharing its CFG denoiser when ws >= 2)
             use_pair = cond_free and ws >= 2 and os.environ.get("TTB_CFG_PAIR", "1") == "1"   # TTB_CFG_PAIR=0 disables
             groups, _ = parallel.pair_groups() if use_pair else (None, 0)
@@ -515,7 +627,7 @@ class TextToSpeech:
                     wavs[j] = self.vocoder.inference(mel, z)
                 e[3].record()
                 timers.append(e)
-            ev[3].record()
+            ev[2].record()
             t_red = None
             if self.enable_redaction and text is not None and "[" in text:
                 # api.py:583-587: every candidate this rank rendered, before the waveforms are exchanged
@@ -539,12 +651,7 @@ class TextToSpeech:
                 res.append(w.reshape(1, 1, -1).cpu())          # wav.cpu() synchronises, as in the reference
             for e in timers:
                 t_lat += e[0].elapsed_time(e[1]); t_diff += e[1].elapsed_time(e[2]); t_voc += e[2].elapsed_time(e[3])
-            self.last_timings = {"ar_ms": ev[0].elapsed_time(ev[1]), "clvp_ms": ev[1].elapsed_time(ev[2]),
-                                 "latents_ms": t_lat, "diffusion_ms": t_diff, "vocoder_ms": t_voc,
-                                 "device_total_ms": ev[0].elapsed_time(ev[3])}
+            t = {"latents_ms": t_lat, "diffusion_ms": t_diff, "vocoder_ms": t_voc}
             if t_red is not None:
-                self.last_timings["redaction_ms"] = t_red
-        out = res if len(res) > 1 else res[0]
-        if return_deterministic_state:
-            return out, (seed, text, voice_samples, conditioning_latents)
-        return out
+                t["redaction_ms"] = t_red
+        return res, t

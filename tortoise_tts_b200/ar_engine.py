@@ -19,6 +19,44 @@ def _f(t, dev):
     return t.to(device=dev, dtype=torch.float32).contiguous()
 
 
+def plan_batches(utterances, max_rows=lib.AR_STEP_MAX_B, max_groups=lib.AR_STEP_MAX_GROUPS, max_P=lib.AR_STEP_MAX_P):
+    """Packs utterances into consecutive decode batches for AREngine.generate_grouped. `utterances`: list of
+    (candidates, prompt positions P). Returns a list of batches, each a list of utterance indices in order; an utterance
+    is never split. A batch holds at most `max_rows` candidates and `max_groups` utterances. An utterance with more than
+    `max_rows` candidates or a prompt longer than `max_P` positions is a batch of its own (decoded by generate())."""
+    batches, cur, rows = [], [], 0
+    for u, (n, P) in enumerate(utterances):
+        n, P = int(n), int(P)
+        if n <= 0 or P <= 0:
+            raise ValueError("utterance %d: %d candidates, prompt of %d positions" % (u, n, P))
+        if n > max_rows or P > max_P:
+            if cur:
+                batches.append(cur)
+            batches.append([u])
+            cur, rows = [], 0
+            continue
+        if cur and (rows + n > max_rows or len(cur) == max_groups):
+            batches.append(cur)
+            cur, rows = [], 0
+        cur.append(u)
+        rows += n
+    if cur:
+        batches.append(cur)
+    return batches
+
+
+def clip_groups(groups, lo, hi):
+    """The prompt groups [(row_begin, row_end, P, prefix), ...] of a batch as seen by the decode chain of rows [lo, hi):
+    groups that overlap the chain, clipped to it, with rows counted from lo. A group that straddles two chains appears
+    in both and shares its (read-only) prefix."""
+    out = []
+    for b, e, P, pkv in groups:
+        b2, e2 = max(b, lo), min(e, hi)
+        if b2 < e2:
+            out.append((b2 - lo, e2 - lo, P, pkv))
+    return out
+
+
 class ARWeights:
     """Packs `autoregressive.pth` (SURVEY App. B): HF Conv1D weights [in,out] are transposed to K-major bf16."""
 
@@ -136,20 +174,50 @@ class AREngine:
         lib.gemm(st["hn"], self.w.w_head, M=1, N=self.V, K=D, bias=self.w.b_head, out_f32=st["logits"])
 
     # ------------------------------------------------------------------ decode workspace + graph
-    def _decode_state(self, B, P, Nmax):
-        key = (B, P, Nmax)
+    def _decode_state(self, B, P, Nmax, group_rows=None, group_P=None):
+        """Decode workspace of B candidates. group_rows / group_P (grouped decode): the candidates of each utterance of the
+        batch and its prompt length; P is then unused and every group gets its own prefix buffers (st["groups"])."""
+        key = (B, P, Nmax) if group_rows is None else (B, tuple(group_rows), tuple(group_P), Nmax)
         if self._dec is not None and self._dec["key"] == key:
             return self._dec
         self._dec = None                  # release the previous workspace (KV caches) before allocating the next
-        cfg, D, dev = self.cfg, self.D, self.dev
-        ok = lib.ar_step_supported(B, D, self.H, P)
+        dev = self.dev
+        if group_rows is None:
+            ok = lib.ar_step_supported(B, self.D, self.H, P)
+        else:
+            ok = all(lib.ar_step_supported(B, self.D, self.H, p) for p in group_P)
+            if not ok or self.MODE == "perop" or len(group_rows) > lib.AR_STEP_MAX_GROUPS:
+                raise lib.TtbError("grouped decode needs the one-kernel step: %d groups (at most %d), %d rows, prompts %s "
+                                   "(mode %s)" % (len(group_rows), lib.AR_STEP_MAX_GROUPS, B, list(group_P), self.MODE))
         mode = self.MODE if ok else "perop"
         if mode == "auto":
             mode = "fused" if B <= self.FUSED_MAX_B else "mixed"
         nch = self.CHAINS if (mode == "mixed" and self.CHAINS > 1 and B >= self.CHAINS_MIN_B and B % self.CHAINS == 0) else 1
         st = dict(key=key, P=P, B=B, Nmax=Nmax, mode=mode, fused=mode in ("fused", "mixed"))
+        if group_rows is None:
+            # ---- prompt prefill (shared by every candidate and every chain)
+            self._prefix_state(st, P)
+        else:
+            st["groups"] = []
+            b = 0
+            for n, p in zip(group_rows, group_P):
+                gs = dict(P=p, fused=True, b0=b, b1=b + n)
+                self._prefix_state(gs, p)
+                st["groups"].append(gs)
+                b += n
+        # ---- decode workspaces: one per chain (contiguous candidate ranges)
+        per = B // nch
+        st["chains"] = [self._chain_state(st, per, c * per, compact=nch > 1) for c in range(nch)]
+        st["sides"] = [torch.cuda.Stream(device=dev) for _ in range(nch - 1)] if dev.type == "cuda" else []
+        st["graph"] = None
+        st["graph_params"] = None
+        self._dec = st
+        return st
+
+    def _prefix_state(self, st, P):
+        """Prefill buffers and the prompt-prefix KV cache of one prompt of P positions, into the dict `st`."""
+        cfg, D, dev = self.cfg, self.D, self.dev
         L, H = cfg.ar_layers, self.H
-        # ---- prompt prefill (shared by every candidate and every chain)
         st["px"] = torch.empty(P, D, dtype=torch.float32, device=dev)
         st["pws"] = self._alloc_trunk(P)
         if st["fused"]:
@@ -160,21 +228,18 @@ class AREngine:
             st["pv"] = torch.empty(L, H, P, 64, dtype=torch.bfloat16, device=dev)
         st["hn"] = torch.empty(1, D, dtype=torch.bfloat16, device=dev)
         st["logits"] = torch.empty(1, self.V, dtype=torch.float32, device=dev)
-        # ---- decode workspaces: one per chain (contiguous candidate ranges)
-        per = B // nch
-        st["chains"] = [self._chain_state(st, per, c * per, compact=nch > 1) for c in range(nch)]
-        st["sides"] = [torch.cuda.Stream(device=dev) for _ in range(nch - 1)] if dev.type == "cuda" else []
-        st["graph"] = None
-        st["graph_params"] = None
-        self._dec = st
-        return st
 
     def _chain_state(self, st, B, b0, compact=False):
         """Decode workspace of candidates [b0, b0 + B): residual stream, trunk buffers, candidate KV cache, sampler state."""
         cfg, D, H, dev = self.cfg, self.D, self.H, self.dev
         L, Nmax = cfg.ar_layers, st["Nmax"]
         ch = dict(B=B, b0=b0, P=st["P"], Nmax=Nmax, mode=st["mode"], fused=st["fused"], compact=compact)
-        if st["fused"]:
+        if "groups" in st:
+            ch["groups"] = clip_groups([(g["b0"], g["b1"], g["P"], g["pkv"]) for g in st["groups"]], b0, b0 + B)
+            ch["P"] = max(g[2] for g in ch["groups"])
+            ch["pkv"] = ch["groups"][0][3]
+            ch["ckv"] = torch.zeros(L, B, H, Nmax, 2, 64, dtype=torch.bfloat16, device=dev)
+        elif st["fused"]:
             ch["pkv"] = st["pkv"]
             ch["ckv"] = torch.zeros(L, B, H, Nmax, 2, 64, dtype=torch.bfloat16, device=dev)
         else:
@@ -207,7 +272,7 @@ class AREngine:
                             lnf_b=w.lnf_b, fn_g=w.fn_g, fn_b=w.fn_b, mel_emb=w.mel_emb, mel_pos=w.mel_pos,
                             codes=st["codes"], ld_codes=st["Nmax"], state=st["state"], x=st["x"], a=ws["a"], qkv=ws["qkv"],
                             o=ws["o"], h=ws["h"], hn=st["hn"], logits=st["logits"], prefix_kv=st["pkv"], cand_kv=st["ckv"],
-                            attn_compact=bool(st.get("compact")))
+                            attn_compact=bool(st.get("compact")), groups=st.get("groups"))
             st["step_handles"][pos_mode] = hd
         return hd
 
@@ -296,17 +361,47 @@ class AREngine:
         self._prefill(cond_latent, text_tokens, st)
         if trace_logits is not None:   # parity hook (eager mode): logits the sampler sees at every step
             trace_logits.append(st["logits"][:1].expand(B, -1).clone())
-        w, bit = divmod(cfg.start_mel_token, 32)
         for ch in st["chains"]:
-            ch["uniforms"].copy_(uniforms[ch["b0"]: ch["b0"] + ch["B"]])
-            ch["state"].zero_()
-            ch["finished"].zero_()
-            ch["codes"].fill_(cfg.stop_mel_token)
-            ch["seen"].zero_()
-            # HF's repetition penalty sees the fake prompt ids {1, start_mel} (autoregressive.py:546-548)
-            ch["seen"][:, 0] = 2
-            ch["seen"][:, w] |= (1 << bit) if bit < 31 else -(1 << 31)
+            self._reset_chain(ch, uniforms)
             self._sample(sp, st["logits"], 0, ch)
+        return st
+
+    def _reset_chain(self, ch, uniforms):
+        """Sampler state of one chain before the first token; `uniforms` [B, Nmax] of the whole batch."""
+        cfg = self.cfg
+        w, bit = divmod(cfg.start_mel_token, 32)
+        ch["uniforms"].copy_(uniforms[ch["b0"]: ch["b0"] + ch["B"]])
+        ch["state"].zero_()
+        ch["finished"].zero_()
+        ch["codes"].fill_(cfg.stop_mel_token)
+        ch["seen"].zero_()
+        # HF's repetition penalty sees the fake prompt ids {1, start_mel} (autoregressive.py:546-548)
+        ch["seen"][:, 0] = 2
+        ch["seen"][:, w] |= (1 << bit) if bit < 31 else -(1 << 31)
+
+    def _begin_grouped(self, cond_latent, text_tokens_list, counts, Nmax, uniforms_list, seed, sp, trace_logits=None):
+        """_begin for a batch of utterances: one prefill per utterance into its own prefix, and the first token of every
+        row sampled from its utterance's prefill logits (one sampler call per chain, so the step counter advances once)."""
+        dev = self.dev
+        Ps = [len(t) + 4 for t in text_tokens_list]
+        st = self._decode_state(sum(counts), None, Nmax, counts, Ps)
+        us = []
+        for n, u in zip(counts, uniforms_list if uniforms_list is not None else [None] * len(counts)):
+            if u is None:          # as generate(): every utterance draws its own table from the same seed
+                g = torch.Generator(device=dev)
+                g.manual_seed(0 if seed is None else int(seed))
+                u = torch.rand(n, Nmax, generator=g, device=dev)
+            us.append(u.to(device=dev, dtype=torch.float32))
+        uniforms = torch.cat(us, dim=0)
+        for gs, toks in zip(st["groups"], text_tokens_list):
+            self._prefill(cond_latent, toks, gs)
+        first = torch.cat([gs["logits"].expand(gs["b1"] - gs["b0"], -1) for gs in st["groups"]], dim=0)
+        if trace_logits is not None:
+            trace_logits.append(first.clone())
+        for ch in st["chains"]:
+            self._reset_chain(ch, uniforms)
+            ch["logits"].copy_(first[ch["b0"]: ch["b0"] + ch["B"]])
+            self._sample(sp, ch["logits"], self.V, ch)
         return st
 
     _SNAP = ("state", "codes", "seen", "finished")
@@ -379,7 +474,32 @@ class AREngine:
         if trace_logits is not None:
             use_graph = False
         st = self._begin(cond_latent, text_tokens, B, Nmax, uniforms, seed, sp, trace_logits)
-        steps = Nmax - 1
+        self._decode(st, sp, Nmax - 1, use_graph, stop_check_every, trace_logits)
+        return self._codes(st)
+
+    def generate_grouped(self, cond_latent, text_tokens_list, counts, max_new, uniforms_list=None, seed=None,
+                         temperature=0.8, top_k=50, top_p=0.8, repetition_penalty=2.0, pos_mode="ref_kv_quirk",
+                         use_graph=True, stop_check_every=32, trace_logits=None, typical_mass=None):
+        """Several utterances decoded in ONE batch: utterance u contributes counts[u] candidates that attend to its own
+        prompt (text_tokens_list[u], one shared conditioning latent). Returns one int32 codes tensor [counts[u], max_new]
+        per utterance, each as generate(cond_latent, text_tokens_list[u], counts[u], max_new, uniforms_list[u], ...)
+        returns it. At most lib.AR_STEP_MAX_GROUPS utterances, lib.AR_STEP_MAX_B rows and prompts of
+        lib.AR_STEP_MAX_P positions (plan_batches packs within these limits); the one-kernel step is required."""
+        counts = [int(n) for n in counts]
+        if len(counts) != len(text_tokens_list) or (uniforms_list is not None and len(uniforms_list) != len(counts)):
+            raise ValueError("one entry of counts (and of uniforms_list) per utterance")
+        Nmax = int(max_new)
+        sp = self._sampling(temperature, top_k, top_p, repetition_penalty, pos_mode, typical_mass)
+        if trace_logits is not None:
+            use_graph = False
+        st = self._begin_grouped(cond_latent, text_tokens_list, counts, Nmax, uniforms_list, seed, sp, trace_logits)
+        self._decode(st, sp, Nmax - 1, use_graph, stop_check_every, trace_logits)
+        codes = self._codes(st)
+        return [codes[g["b0"]: g["b1"]].clone() for g in st["groups"]]
+
+    def _decode(self, st, sp, steps, use_graph, stop_check_every, trace_logits):
+        """The decode loop after the first token: `steps` steps (graph replays polled for the stop every
+        stop_check_every steps, or eager with the logits traced)."""
         if steps > 0:
             if use_graph:
                 self._ensure_graph(st, sp)
@@ -399,7 +519,6 @@ class AREngine:
                         trace_logits.append(torch.cat([ch["logits"] for ch in st["chains"]], dim=0).clone())
         if st["fused"] and steps > 0:
             self._check_step_flag(st)
-        return self._codes(st)
 
     def generate_stream(self, cond_latent, text_tokens, max_new, first_block, block, uniforms=None, seed=None,
                         temperature=0.8, top_k=50, top_p=0.8, repetition_penalty=2.0, pos_mode="ref_kv_quirk",

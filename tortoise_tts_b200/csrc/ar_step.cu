@@ -46,6 +46,7 @@ constexpr int AS_MAX_TILES = 512;                          // ticket counters (r
 constexpr int AS_SYNC_BAR_BYTES = 17 * 128;                // barrier epoch line + 16 arrival-counter lines
 constexpr int AS_COMPACT_WARPS = 8;                        // ar_attn_compact_kernel: 256 threads, ~118 KB at P = 174
 constexpr int AS_COMPACT_CTAS = 2;                         // ar_attn_compact_kernel CTAs per SM
+constexpr int AS_MAX_GROUPS = 16;                          // prompt-prefix groups of one step (TtbArStepArgs.groups)
 
 enum { G_QKV = 0, G_PROJ = 1, G_FC = 2, G_PROJ2 = 3, G_HEAD = 4 };
 enum { OUT_PARTIAL = 0, OUT_BF16 = 1, OUT_F32 = 2 };
@@ -58,10 +59,18 @@ struct AsLayer {       // device table, one per layer
   const float *ln1_g, *ln1_b, *bqkv, *bproj, *ln2_g, *ln2_b, *bfc, *bproj2;
 };
 
+// One prompt-prefix group of the attention phase: rows [b0, next b0) attend to a prefix of P positions (tensor map
+// maps[4 L + 6 + g]); its attention units are [u0, next u0), ncph CTAs per head. Entry [groups] is a sentinel whose
+// b0 is B and whose u0 is the total number of units.
+struct AsGroup {
+  int b0, P, u0, ncph;
+};
+
 struct AsParams {
-  int B, D, H, L, V, P, Nmax, pos_mode;
+  int B, D, H, L, V, Nmax, pos_mode;
   int TB, nbt, nst, stage_bytes;          // batch tile (wgmma N), number of batch tiles, pipeline stages
-  int ncph, ipr, team;                    // attention: CTAs per head, items per round, warps per item
+  int units, ipr, team;                   // attention: work units (group, head, chunk), items per round, warps per item
+  AsGroup gtab[AS_MAX_GROUPS + 1];        // [groups + 1] (one group when every row shares one prompt)
   int layer_begin, layer_end, phase_mask; // debug / profiling: subset of the step (phase_mask bit i = phase i of a layer)
   AsGemmShape g[5];
   const CUtensorMap* maps;                // device: [4*L + 1] weight maps, then activation maps a, o, h, hn
@@ -75,7 +84,7 @@ struct AsParams {
   __nv_bfloat16 *a, *qkv, *o, *h, *hn;
   float* part;
   float* logits;
-  const __nv_bfloat16* prefix_kv;         // [L][H][P][2][64]
+  const __nv_bfloat16* prefix_kv;         // [L][H][P][2][64] (group 0)
   __nv_bfloat16* cand_kv;                 // [L][B][H][Nmax][2][64]
   unsigned long long* bar;                // [0] barrier epoch at launch; arrival slots at [16 * (1 + k)], k < 16
   unsigned int* tickets;                  // [AS_MAX_TILES]
@@ -489,7 +498,7 @@ template <class CtrlT>
 TTB_DEVINL void attn_phase_mma(const AsParams& p, int layer, uint8_t* data, CtrlT* ctrl, AsRole& rl, bool wait_pdl = false) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   int* err = &p.state->reserved[0];
-  const int B = p.B, H = p.H, P = p.P, Nmax = p.Nmax, D = p.H * 64;
+  const int B = p.B, H = p.H, Nmax = p.Nmax, D = p.H * 64;
   constexpr int NS = AS_RING_NS;
   constexpr int CHUNK_BYTES = AS_CHUNK_BYTES;          // K tile 2 KB | V tile 2 KB
   const int slot = p.state->step - 1;
@@ -497,13 +506,17 @@ TTB_DEVINL void attn_phase_mma(const AsParams& p, int layer, uint8_t* data, Ctrl
   uint8_t* ring = data + warp * NS * CHUNK_BYTES;
   uint8_t* prefix_s = data + p.ipr * p.team * NS * CHUNK_BYTES;   // behind the rings of the active warps (host checks the fit)
   const CUtensorMap* map_c = p.maps + 4 * p.L + 5;
-  const CUtensorMap* map_p = map_c + 1;
   __nv_bfloat16* ckv_l = p.cand_kv + (long long)layer * B * H * Nmax * 128;
-  const int npc = (P + 15) / 16;
-  const int units = H * p.ncph;
-  for (int u = blockIdx.x; u < units; u += gridDim.x) {
-    const int h = u % H, ci = u / H;
-    const int b_begin = (int)((long long)ci * B / p.ncph), b_end = (int)((long long)(ci + 1) * B / p.ncph);
+  int g = 0;
+  for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
+    while (u >= p.gtab[g + 1].u0) ++g;                   // a CTA's units only grow: its group only advances
+    const int gb0 = p.gtab[g].b0, gB = p.gtab[g + 1].b0 - gb0, ncph = p.gtab[g].ncph;
+    const int P = p.gtab[g].P;
+    const CUtensorMap* map_p = map_c + 1 + g;            // prompt prefix of this unit's group
+    const int npc = (P + 15) / 16;
+    const int lu = u - p.gtab[g].u0;
+    const int h = lu % H, ci = lu / H;
+    const int b_begin = gb0 + (int)((long long)ci * gB / ncph), b_end = gb0 + (int)((long long)(ci + 1) * gB / ncph);
     __syncthreads();
     if (threadIdx.x == 0) {
       mbar_arrive_expect_tx(&ctrl->prefix_bar, (uint32_t)(npc * CHUNK_BYTES));
@@ -882,6 +895,7 @@ struct AsPlan {
   AsParams p;
   long long part_floats;
   int grid;
+  int ngroups;                            // >= 1 (groups == 0 is one group of every row)
 };
 
 static int as_num_sms() {
@@ -914,11 +928,33 @@ static int make_plan(const TtbArStepArgs& a, AsPlan& pl) {
   memset(&p, 0, sizeof(p));
   if (a.B <= 0 || a.B > 256) { set_error("ttb_ar_step: B=%d unsupported (1..256)", a.B); return -1; }
   if (a.D != a.H * 64 || a.D % 128 != 0 || a.D > 1024) { set_error("ttb_ar_step: D=%d H=%d unsupported (D = 64 H, D %% 128 == 0, D <= 1024)", a.D, a.H); return -1; }
-  if (a.P <= 0 || a.P > AS_MAX_P) { set_error("ttb_ar_step: prompt length P=%d exceeds %d", a.P, AS_MAX_P); return -1; }
+  if (a.groups < 0 || a.groups > AS_MAX_GROUPS) { set_error("ttb_ar_step: %d prompt groups (0..%d)", a.groups, AS_MAX_GROUPS); return -1; }
+  // prompt groups: rows [group_begin[g], group_begin[g + 1]) share the prefix group_prefix_kv[g] of group_P[g] positions
+  pl.ngroups = a.groups > 0 ? a.groups : 1;
+  if (a.groups > 0) {
+    if (!a.group_begin || !a.group_P || !a.group_prefix_kv) { set_error("ttb_ar_step: missing group arrays"); return -1; }
+    if (a.group_begin[0] != 0 || a.group_begin[a.groups] != a.B) {
+      set_error("ttb_ar_step: groups must cover rows [0, B=%d)", a.B); return -1;
+    }
+    for (int g = 0; g < a.groups; ++g) {
+      if (a.group_begin[g + 1] <= a.group_begin[g]) { set_error("ttb_ar_step: group %d has no rows", g); return -1; }
+      if (!a.group_prefix_kv[g]) { set_error("ttb_ar_step: group %d has no prefix", g); return -1; }
+      p.gtab[g].b0 = a.group_begin[g]; p.gtab[g].P = a.group_P[g];
+    }
+  } else {
+    p.gtab[0].b0 = 0; p.gtab[0].P = a.P;
+  }
+  p.gtab[pl.ngroups].b0 = a.B;
+  int maxP = 0;
+  for (int g = 0; g < pl.ngroups; ++g) {
+    const int P = p.gtab[g].P;
+    if (P <= 0 || P > AS_MAX_P) { set_error("ttb_ar_step: prompt length P=%d exceeds %d", P, AS_MAX_P); return -1; }
+    if (P > maxP) maxP = P;
+  }
   if (a.L <= 0 || a.V <= 0 || a.Nmax <= 0) { set_error("ttb_ar_step: bad shape"); return -1; }
   const int grid = as_num_sms();
   pl.grid = grid;
-  p.B = a.B; p.D = a.D; p.H = a.H; p.L = a.L; p.V = a.V; p.P = a.P; p.Nmax = a.Nmax; p.pos_mode = a.pos_mode;
+  p.B = a.B; p.D = a.D; p.H = a.H; p.L = a.L; p.V = a.V; p.Nmax = a.Nmax; p.pos_mode = a.pos_mode;
   const int Bpad = (a.B + 15) & ~15;
   p.nbt = (Bpad + 127) / 128;
   p.TB = (((Bpad + p.nbt - 1) / p.nbt) + 15) & ~15;
@@ -940,11 +976,23 @@ static int make_plan(const TtbArStepArgs& a, AsPlan& pl) {
     if (p.g[i].n_rt * p.nbt > AS_MAX_TILES) { set_error("ttb_ar_step: too many tiles"); return -1; }
   }
   pl.part_floats = pf;
-  // attention decomposition (compact attention: AS_COMPACT_CTAS CTAs per SM, see ar_attn_compact_kernel)
-  p.ncph = grid * (a.attn_compact ? AS_COMPACT_CTAS : 1) / a.H;
-  if (p.ncph < 1) p.ncph = 1;
-  if (p.ncph > a.B) p.ncph = a.B;
-  const int max_items = (a.B + p.ncph - 1) / p.ncph;
+  // attention decomposition (compact attention: AS_COMPACT_CTAS CTAs per SM, see ar_attn_compact_kernel): units =
+  // (group, head, chunk of the group's rows); the CTAs per head are shared out over the groups in proportion to their rows
+  const int ncph = grid * (a.attn_compact ? AS_COMPACT_CTAS : 1) / a.H;
+  int max_items = 1;
+  p.units = 0;
+  for (int g = 0; g < pl.ngroups; ++g) {
+    AsGroup& gr = p.gtab[g];
+    const int gB = p.gtab[g + 1].b0 - gr.b0;
+    gr.ncph = (int)((long long)ncph * gB / a.B);
+    if (gr.ncph < 1) gr.ncph = 1;
+    if (gr.ncph > gB) gr.ncph = gB;
+    gr.u0 = p.units;
+    p.units += a.H * gr.ncph;
+    const int items = (gB + gr.ncph - 1) / gr.ncph;
+    if (items > max_items) max_items = items;
+  }
+  p.gtab[pl.ngroups].u0 = p.units;
   const int wcap = a.attn_compact ? AS_COMPACT_WARPS : AS_WARPS;
   const int rounds = (max_items + wcap - 1) / wcap;
   p.ipr = (max_items + rounds - 1) / rounds;
@@ -955,12 +1003,12 @@ static int make_plan(const TtbArStepArgs& a, AsPlan& pl) {
   const int tcap = env_int("TTB_AR_STEP_TEAM", 0);
   if (tcap > 0 && tcap < team) team = tcap;
   p.team = team;
-  // the rings of the active warps + the prompt prefix of one head share the data region
+  // the rings of the active warps + the longest prompt prefix of one head share the data region
   const int nact = p.ipr * p.team;
-  const long long attn_bytes = (long long)nact * AS_RING_NS * AS_CHUNK_BYTES + (long long)((a.P + 15) & ~15) * AS_POS_BYTES;
+  const long long attn_bytes = (long long)nact * AS_RING_NS * AS_CHUNK_BYTES + (long long)((maxP + 15) & ~15) * AS_POS_BYTES;
   if (attn_bytes > AS_DATA_BYTES) {
     set_error("ttb_ar_step: ring %d x %d positions x %d warps + prompt %d do not fit shared memory", AS_RING_NS, AS_CHUNK_POS,
-              nact, a.P);
+              nact, maxP);
     return -1;
   }
   p.attn_data_bytes = a.attn_compact ? (int)((attn_bytes + 1023) & ~1023LL) : 0;
@@ -970,9 +1018,11 @@ static int make_plan(const TtbArStepArgs& a, AsPlan& pl) {
   return 0;
 }
 
-constexpr int AS_EXTRA_MAPS = 6;      // activations a, o, h, hn; candidate KV cache; prompt-prefix KV cache
-static long long table_bytes(int L) {
-  return (long long)(4 * L + 1 + AS_EXTRA_MAPS) * sizeof(CUtensorMap) + (long long)L * sizeof(AsLayer) + 256;
+constexpr int AS_EXTRA_MAPS = 6;      // activations a, o, h, hn; candidate KV cache; prompt-prefix KV cache of group 0
+// device tables: tensor maps (weights, extra maps, the prefixes of groups 1..), layer table
+static int num_maps(int L, int ngroups) { return 4 * L + 1 + AS_EXTRA_MAPS + (ngroups - 1); }
+static long long table_bytes(int L, int ngroups) {
+  return (long long)num_maps(L, ngroups) * sizeof(CUtensorMap) + (long long)L * sizeof(AsLayer) + 256;
 }
 
 }  // namespace ttb
@@ -983,7 +1033,7 @@ extern "C" int ttb_ar_step_workspace(const TtbArStepArgs* a, long long* part_flo
   AsPlan pl;
   if (make_plan(*a, pl)) return -1;
   if (part_floats) *part_floats = pl.part_floats;
-  if (table_bytes_out) *table_bytes_out = table_bytes(a->L);
+  if (table_bytes_out) *table_bytes_out = table_bytes(a->L, pl.ngroups);
   if (sync_bytes) *sync_bytes = AS_SYNC_BAR_BYTES + AS_MAX_TILES * 4;
   return 0;
 }
@@ -996,8 +1046,8 @@ extern "C" int ttb_ar_step_setup(const TtbArStepArgs* ap, void* stream) {
   AsPlan pl;
   if (make_plan(a, pl)) return -1;
   if (!a.layers || !a.tables || !a.sync) { set_error("ttb_ar_step_setup: missing tables"); return -1; }
-  const int nmaps = 4 * a.L + 1 + AS_EXTRA_MAPS;
-  std::vector<unsigned char> host((size_t)table_bytes(a.L), 0);
+  const int nmaps = num_maps(a.L, pl.ngroups);
+  std::vector<unsigned char> host((size_t)table_bytes(a.L, pl.ngroups), 0);
   CUtensorMap* maps = reinterpret_cast<CUtensorMap*>(host.data());
   AsLayer* lay = reinterpret_cast<AsLayer*>(host.data() + (size_t)nmaps * sizeof(CUtensorMap));
   const uint64_t D = a.D;
@@ -1024,9 +1074,14 @@ extern "C" int ttb_ar_step_setup(const TtbArStepArgs* ap, void* stream) {
     const uint64_t cd[4] = {64, 2, (uint64_t)a.Nmax, (uint64_t)a.L * a.B * a.H};
     const uint64_t cs[3] = {128, 256, (uint64_t)a.Nmax * 256};
     if (make_tensor_map_bf16_nd(&am[4], a.cand_kv, 4, cd, cs, box)) return -1;
-    const uint64_t pd[4] = {64, 2, (uint64_t)a.P, (uint64_t)a.L * a.H};
-    const uint64_t ps[3] = {128, 256, (uint64_t)a.P * 256};
-    if (make_tensor_map_bf16_nd(&am[5], a.prefix_kv, 4, pd, ps, box)) return -1;
+    // prompt prefix of group g, [L][H][P_g][2][64]: maps[4 L + 6 + g]
+    for (int g = 0; g < pl.ngroups; ++g) {
+      const uint64_t P = (uint64_t)pl.p.gtab[g].P;
+      const uint64_t pd[4] = {64, 2, P, (uint64_t)a.L * a.H};
+      const uint64_t ps[3] = {128, 256, P * 256};
+      const void* pkv = a.groups > 0 ? a.group_prefix_kv[g] : a.prefix_kv;
+      if (make_tensor_map_bf16_nd(&am[5 + g], pkv, 4, pd, ps, box)) return -1;
+    }
   }
   cudaError_t e = cudaMemcpyAsync(a.tables, host.data(), host.size(), cudaMemcpyHostToDevice, st);
   if (e == cudaSuccess) e = cudaMemsetAsync(a.sync, 0, AS_SYNC_BAR_BYTES + AS_MAX_TILES * 4, st);
@@ -1049,7 +1104,7 @@ extern "C" int ttb_ar_decode_step(const TtbArStepArgs* ap, void* stream) {
   AsPlan pl;
   if (make_plan(a, pl)) return -1;
   AsParams& p = pl.p;
-  const int nmaps = 4 * a.L + 1 + AS_EXTRA_MAPS;
+  const int nmaps = num_maps(a.L, pl.ngroups);
   p.maps = reinterpret_cast<const CUtensorMap*>(a.tables);
   p.layers = reinterpret_cast<const AsLayer*>(reinterpret_cast<const unsigned char*>(a.tables) + (size_t)nmaps * sizeof(CUtensorMap));
   p.lnf_g = a.lnf_g; p.lnf_b = a.lnf_b; p.fn_g = a.fn_g; p.fn_b = a.fn_b; p.b_head = a.b_head;
@@ -1064,7 +1119,7 @@ extern "C" int ttb_ar_decode_step(const TtbArStepArgs* ap, void* stream) {
   p.bar = reinterpret_cast<unsigned long long*>(a.sync);
   p.tickets = reinterpret_cast<unsigned int*>(reinterpret_cast<unsigned char*>(a.sync) + AS_SYNC_BAR_BYTES);
   if (p.phase_mask == PH_ATTN && p.layer_end == p.layer_begin + 1) {
-    const int units = a.H * p.ncph;
+    const int units = p.units;
     if (a.attn_compact) {
       const int cgrid = pl.grid * AS_COMPACT_CTAS;
       const cudaError_t lc = launch_pdl(ar_attn_compact_kernel, dim3(units < cgrid ? units : cgrid), dim3(AS_COMPACT_WARPS * 32),

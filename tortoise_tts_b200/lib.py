@@ -62,7 +62,9 @@ class ArStepArgs(C.Structure):
                 ("h", C.c_void_p), ("hn", C.c_void_p), ("part", C.c_void_p), ("logits", C.c_void_p),
                 ("prefix_kv", C.c_void_p), ("cand_kv", C.c_void_p), ("tables", C.c_void_p), ("sync", C.c_void_p),
                 ("debug_layer_begin", C.c_int), ("debug_layer_end", C.c_int), ("debug_phase_mask", C.c_int),
-                ("attn_compact", C.c_int)]
+                ("attn_compact", C.c_int),
+                ("groups", C.c_int), ("group_begin", C.POINTER(C.c_int)), ("group_P", C.POINTER(C.c_int)),
+                ("group_prefix_kv", C.POINTER(C.c_void_p))]
 
 
 _lib = None
@@ -228,6 +230,7 @@ def ar_step_store_prefix(qkv, P, H, pkv):
 
 
 AR_STEP_MAX_B, AR_STEP_MAX_P, AR_STEP_MAX_D = 256, 352, 1024    # limits of csrc/ar_step.cu (make_plan)
+AR_STEP_MAX_GROUPS = 16                                          # prompt groups of one step (TtbArStepArgs.groups)
 
 
 def ar_step_supported(B, D, H, P):
@@ -236,13 +239,16 @@ def ar_step_supported(B, D, H, P):
 
 class ArStep:
     """Handle of the one-kernel decode step (include/ttb.h TtbArStepArgs): owns the scratch / table / sync buffers and
-    keeps every tensor the kernel points at alive. `layers`: list of dicts with the keys of ARWeights.layers."""
+    keeps every tensor the kernel points at alive. `layers`: list of dicts with the keys of ARWeights.layers.
+    `groups`: None (every row attends to `prefix_kv` of P positions) or a list of (row_begin, row_end, P_g, prefix_kv_g)
+    covering rows [0, B) in order; `P` and `prefix_kv` are then ignored."""
 
     def __init__(self, *, B, D, H, L, V, P, Nmax, pos_mode, layers, w_head, b_head, lnf_g, lnf_b, fn_g, fn_b, mel_emb,
-                 mel_pos, codes, ld_codes, state, x, a, qkv, o, h, hn, logits, prefix_kv, cand_kv, attn_compact=False):
+                 mel_pos, codes, ld_codes, state, x, a, qkv, o, h, hn, logits, prefix_kv, cand_kv, attn_compact=False,
+                 groups=None):
         dev = x.device
         self._keep = (layers, w_head, b_head, lnf_g, lnf_b, fn_g, fn_b, mel_emb, mel_pos, codes, state, x, a, qkv, o, h,
-                      hn, logits, prefix_kv, cand_kv)
+                      hn, logits, prefix_kv, cand_kv, groups)
         self._larr = (ArStepLayer * L)()
         for i, lw in enumerate(layers):
             for n in ("wqkv", "wproj", "wfc", "wproj2"):
@@ -260,6 +266,15 @@ class ArStep:
         g.h, g.hn, g.logits = _bf(h).data_ptr(), _bf(hn).data_ptr(), _f32(logits).data_ptr()
         g.prefix_kv, g.cand_kv = _bf(prefix_kv).data_ptr(), _bf(cand_kv).data_ptr()
         g.attn_compact = 1 if attn_compact else 0
+        if groups:
+            n = len(groups)
+            self._gbeg = (C.c_int * (n + 1))(*([int(r[0]) for r in groups] + [int(groups[-1][1])]))
+            self._gP = (C.c_int * n)(*[int(r[2]) for r in groups])
+            self._gkv = (C.c_void_p * n)(*[_bf(r[3]).data_ptr() for r in groups])
+            g.groups = n
+            g.group_begin = C.cast(self._gbeg, C.POINTER(C.c_int))
+            g.group_P = C.cast(self._gP, C.POINTER(C.c_int))
+            g.group_prefix_kv = C.cast(self._gkv, C.POINTER(C.c_void_p))
         pf, tb, sb = C.c_longlong(0), C.c_longlong(0), C.c_longlong(0)
         _chk(load().ttb_ar_step_workspace(C.byref(g), C.byref(pf), C.byref(tb), C.byref(sb)), "ttb_ar_step_workspace")
         self.part = torch.zeros(max(pf.value, 4), dtype=torch.float32, device=dev)
