@@ -213,10 +213,12 @@ typedef struct TtbArStepArgs {
   int attn_compact;                        /* 1: the attention-only launch (debug_phase_mask = 4, one layer) runs in 8-warp CTAs
                                               whose shared memory is sized to the prompt (~118 KB at P = 174), so that CTAs of
                                               another stream fit beside them (two decode chains); same results */
-  /* Prompt groups (several utterances in one batch): groups > 0 (at most 16) replaces prefix_kv / P. Rows
+  /* Prompt groups (several utterances in one batch): groups > 0 (at most 256, one per row) replaces prefix_kv / P. Rows
    * [group_begin[g], group_begin[g + 1]) attend to the prefix group_prefix_kv[g] of group_P[g] positions (<= 352), laid
    * out [L][H][P_g][2][64] as ttb_ar_step_store_prefix writes it; group_begin[0] = 0, group_begin[groups] = B, every
-   * group non-empty. HOST arrays, read by every call that takes these args. groups = 0: every row shares prefix_kv. */
+   * group non-empty. HOST arrays, read by every call that takes these args; ttb_ar_step_setup copies the group table
+   * into `tables` (so a change of groups needs a new setup, as a change of buffers does). groups = 0: every row shares
+   * prefix_kv. */
   int groups;
   const int* group_begin;                  /* [groups + 1] */
   const int* group_P;                      /* [groups] */

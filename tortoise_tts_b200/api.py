@@ -36,6 +36,9 @@ PRESETS = {  # api.py:320-329
     "standard": {"num_autoregressive_samples": 256, "diffusion_iterations": 200},
     "high_quality": {"num_autoregressive_samples": 256, "diffusion_iterations": 400},
 }
+# utterances per decode batch of tts_batch: the step takes up to lib.AR_STEP_MAX_GROUPS prompts, but a larger cap changes
+# which step form decodes some inputs (and so their tokens), which wants its own measurement
+TTS_BATCH_MAX_GROUPS = 16
 
 
 def get_model_path(model_name, models_dir=MODELS_DIR):
@@ -466,7 +469,7 @@ class TextToSpeech:
             g.manual_seed(seed)
             uniforms = torch.rand(B, Nmax, generator=g, device=dev)
             # the grouped step needs the one-kernel step; with the per-op step forced every utterance decodes alone
-            max_groups = 1 if ar.MODE == "perop" else lib.AR_STEP_MAX_GROUPS
+            max_groups = 1 if ar.MODE == "perop" else TTS_BATCH_MAX_GROUPS
             for batch in plan_batches([(B, len(toks[mine[i]]) + 4) for i in range(len(mine))], max_groups=max_groups):
                 us = [mine[i] for i in batch]
                 ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]

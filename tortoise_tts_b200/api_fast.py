@@ -146,15 +146,22 @@ class TextToSpeech:
 
     def _inputs(self, text, voice_samples, text_tokens, use_deterministic_seed):
         seed = self.deterministic_state(seed=use_deterministic_seed)
-        if text_tokens is None:
-            text_tokens = self.tokenizer.encode(text)
-        toks = [int(t) for t in text_tokens] + [0]            # F.pad(text_tokens, (0, 1))
-        assert len(toks) < 400, "Too much text provided. Break the text up into separate segments and re-try inference."
+        toks = self._inputs_tokens(text, text_tokens)
+        return seed, toks, self._auto_latent(voice_samples)
+
+    def _auto_latent(self, voice_samples):
         if voice_samples is not None:
             auto = self.get_conditioning_latents(voice_samples, return_mels=False)
         else:
             auto = self.get_random_conditioning_latents()
-        return seed, toks, auto.to(self.device).float().reshape(-1)
+        return auto.to(self.device).float().reshape(-1)
+
+    def _inputs_tokens(self, text, text_tokens):
+        if text_tokens is None:
+            text_tokens = self.tokenizer.encode(text)
+        toks = [int(t) for t in text_tokens] + [0]            # F.pad(text_tokens, (0, 1))
+        assert len(toks) < 400, "Too much text provided. Break the text up into separate segments and re-try inference."
+        return toks
 
     def _pos_mode(self):
         return "ref_kv_quirk" if self.kv_cache else "train_consistent"
@@ -228,25 +235,130 @@ class TextToSpeech:
         mark = (lambda i: ev[i].record()) if timed else (lambda i: None)
         with torch.no_grad():
             mark(0)
-            g = torch.Generator(device=self.device)
-            g.manual_seed(seed)
-            uniforms = torch.rand(1, n_max, generator=g, device=self.device)
+            uniforms = self._uniforms(seed, n_max)
             codes = self.autoregressive.generate(auto, toks, 1, n_max, uniforms=uniforms, temperature=temperature,
                                                  top_k=top_k, top_p=top_p, repetition_penalty=repetition_penalty,
                                                  pos_mode=self._pos_mode(), use_graph=self.device.type == "cuda",
                                                  typical_mass=typical)
-            hit = (codes[0] == self.cfg.stop_mel_token).nonzero()
-            n = int(hit[0].item()) + 1 if hit.numel() > 0 else n_max          # HF returns the stop token it sampled
-            mark(1)
-            if verbose:
-                print("generating audio..")
-            lat = self.autoregressive.latents(auto, toks, codes[:, :n].contiguous())[0]
-            mark(2)
-            wav = self.hifi_decoder.inference(lat, auto)
-            mark(3)
+            wav, n = self._render(auto, toks, codes, n_max, verbose, mark, 1)
         self.last_timings = {"tokens": n}
         if timed:
             torch.cuda.synchronize()
             self.last_timings = {"ar_ms": ev[0].elapsed_time(ev[1]), "latents_ms": ev[1].elapsed_time(ev[2]),
                              "hifigan_ms": ev[2].elapsed_time(ev[3]), "tokens": n}
-        return wav.reshape(1, 1, -1)
+        return wav
+
+    def _uniforms(self, seed, n_max):
+        """The sampling randomness of one sequence: the first row of a device generator seeded with `seed`."""
+        g = torch.Generator(device=self.device)
+        g.manual_seed(seed)
+        return torch.rand(1, n_max, generator=g, device=self.device)
+
+    def _render(self, auto, toks, codes, n_max, verbose, mark, m0):
+        """What tts() does after the decode, for one sequence `codes` [1, n_max]: cut after the first stop token (HF
+        returns the stop token it sampled), latents over the raw codes, HiFiGAN. `mark(i)` (if given) records event m0
+        after the cut, m0 + 1 after the latents, m0 + 2 after HiFiGAN. Returns (fp32 [1, 1, samples], tokens kept)."""
+        mark = mark or (lambda i: None)
+        hit = (codes[0] == self.cfg.stop_mel_token).nonzero()
+        n = int(hit[0].item()) + 1 if hit.numel() > 0 else n_max
+        mark(m0)
+        if verbose:
+            print("generating audio..")
+        lat = self.autoregressive.latents(auto, toks, codes[:, :n].contiguous())[0]
+        mark(m0 + 1)
+        wav = self.hifi_decoder.inference(lat, auto)
+        mark(m0 + 2)
+        return wav.reshape(1, 1, -1), n
+
+    # ------------------------------------------------------------------ several sentences per call
+    def tts_batch(self, texts, voice_samples=None, text_tokens_list=None, **kwargs):
+        """Several sentences in one call, each ONE sequence: entry u of the returned list is what
+        `tts(texts[u], voice_samples, **kwargs)` returns (fp32 [1, 1, samples] on the device). The conditioning latent
+        and the seed are computed once, and every sentence samples with the uniforms row tts() draws from that seed.
+        The sentences are decoded together: consecutive sentences are packed into decode batches of up to 256 rows,
+        one row per sentence, each attending to its own prompt (ar_engine.plan_batches), so a batch costs about one
+        decode step per token instead of one per sentence and token. A sentence whose prompt is longer than 352
+        positions is decoded alone, as tts() decodes it. The stop-token cut, the latent pass and HiFiGAN then run per
+        sentence as in tts(). `text_tokens_list` (one id list per text) bypasses the tokenizer. `last_timings`: ar_ms
+        (the decode batches, prefills included), prefill_ms (their prompt prefills), latents_ms and hifigan_ms (summed
+        over the sentences), device_total_ms, and tokens (the tokens kept per sentence). Every rank computes the whole
+        batch, as tts() does."""
+        texts = list(texts)
+        if not texts:
+            raise ValueError("tts_batch needs at least one text")
+        if text_tokens_list is not None and len(text_tokens_list) != len(texts):
+            raise ValueError("text_tokens_list has %d entries for %d texts" % (len(text_tokens_list), len(texts)))
+        return self._tts_batch(texts, voice_samples, text_tokens_list, **kwargs)
+
+    def _tts_batch(self, texts, voice_samples, text_tokens_list, k=1, verbose=True, use_deterministic_seed=None,
+                   num_autoregressive_samples=512, temperature=.8, length_penalty=1, repetition_penalty=2.0, top_p=.8,
+                   max_mel_tokens=500, cvvp_amount=.0, top_k=50, typical_sampling=False, typical_mass=.9,
+                   **hf_generate_kwargs):
+        from .ar_engine import plan_batches
+        if hf_generate_kwargs:
+            raise TypeError(f"unsupported generate kwargs: {sorted(hf_generate_kwargs)}")
+        typical = _typical_mass(typical_sampling, typical_mass)
+        seed = self.deterministic_state(seed=use_deterministic_seed)
+        toks = [self._inputs_tokens(texts[u], None if text_tokens_list is None else text_tokens_list[u])
+                for u in range(len(texts))]
+        auto = self._auto_latent(voice_samples)
+        if verbose:
+            print("Generating autoregressive samples..")
+        n_max = self.cfg.max_mel_tokens - 1
+        ar = self.autoregressive
+        timed = self.device.type == "cuda"
+        dec = dict(temperature=temperature, top_k=top_k, top_p=top_p, repetition_penalty=repetition_penalty,
+                   pos_mode=self._pos_mode(), use_graph=timed, typical_mass=typical)
+        new_events = (lambda n: [torch.cuda.Event(enable_timing=True) for _ in range(n)]) if timed else \
+            (lambda n: None)
+        sums = {"ar_ms": 0.0, "prefill_ms": 0.0, "latents_ms": 0.0, "hifigan_ms": 0.0}
+        timed_parts = []                                         # (events, [(key, i, j), ...]) read after one sync
+        wavs, tokens = [None] * len(texts), [0] * len(texts)
+        ends = new_events(2)
+        with torch.no_grad():
+            if timed:
+                ends[0].record()
+            uniforms = self._uniforms(seed, n_max)
+            # the grouped step needs the one-kernel step; with the per-op step forced every sentence decodes alone
+            max_groups = 1 if ar.MODE == "perop" else lib.AR_STEP_MAX_GROUPS
+            for batch in plan_batches([(1, len(t) + 4) for t in toks], max_groups=max_groups):
+                ev = new_events(4)                               # decode start, prefills start / end, decode end
+                pre = (ev[1], ev[2]) if timed else None
+                if timed:
+                    ev[0].record()
+                if len(batch) == 1:
+                    codes = [ar.generate(auto, toks[batch[0]], 1, n_max, uniforms=uniforms, prefill_events=pre, **dec)]
+                else:
+                    codes = ar.generate_grouped(auto, [toks[u] for u in batch], [1] * len(batch), n_max,
+                                                uniforms_list=[uniforms] * len(batch), prefill_events=pre, **dec)
+                if timed:
+                    ev[3].record()
+                    timed_parts.append((ev, [("ar_ms", 0, 3), ("prefill_ms", 1, 2)]))
+                for u, c in zip(batch, codes):
+                    e = new_events(3)
+                    wavs[u], tokens[u] = self._render(auto, toks[u], c, n_max, False,
+                                                      (lambda i, e=e: e[i].record()) if timed else None, 0)
+                    if timed:
+                        timed_parts.append((e, [("latents_ms", 0, 1), ("hifigan_ms", 1, 2)]))
+            if timed:
+                ends[1].record()
+        self.last_timings = {"tokens": tokens}
+        if timed:
+            ends[1].synchronize()
+            for ev, keys in timed_parts:
+                for key, i, j in keys:
+                    sums[key] += ev[i].elapsed_time(ev[j])
+            self.last_timings = {**sums, "device_total_ms": ends[0].elapsed_time(ends[1]), "tokens": tokens}
+        return wavs
+
+    def tts_long(self, text, text_tokens_list=None, **kwargs):
+        """≙ the loop of the reference's `read_fast.py:44-76` for one voice: split the text (`'|'` forces the split
+        points, else `split_and_recombine_text`), render every chunk with the SAME seed and conditioning latent (one
+        tts_batch call), and concatenate the waveforms. Returns `[1, samples]` on the CPU. `text_tokens_list` (one id
+        list per chunk) bypasses the tokenizer; the other keyword arguments are those of tts()."""
+        from .text import split_and_recombine_text
+        texts = text.split("|") if "|" in text else split_and_recombine_text(text)      # read_fast.py:45-51
+        if text_tokens_list is not None and len(text_tokens_list) != len(texts):
+            raise ValueError("text_tokens_list has %d entries for %d chunks" % (len(text_tokens_list), len(texts)))
+        wavs = self.tts_batch(texts, text_tokens_list=text_tokens_list, **kwargs)
+        return torch.cat([w.reshape(1, -1).cpu() for w in wavs], dim=-1)

@@ -348,8 +348,9 @@ class AREngine:
         else:
             lib.ar_sample_typical(*args, sp["typical_mass"], advance=True)
 
-    def _begin(self, cond_latent, text_tokens, B, Nmax, uniforms, seed, sp, trace_logits=None):
-        """Workspace reset + prompt prefill + the first sampled token of every candidate."""
+    def _begin(self, cond_latent, text_tokens, B, Nmax, uniforms, seed, sp, trace_logits=None, prefill_events=None):
+        """Workspace reset + prompt prefill + the first sampled token of every candidate. `prefill_events`: None or a
+        pair of CUDA events recorded around the prefill."""
         cfg, dev = self.cfg, self.dev
         P = len(text_tokens) + 4  # cond + [start, tokens(padded), stop] + start_mel
         st = self._decode_state(B, P, Nmax)
@@ -358,7 +359,11 @@ class AREngine:
             g.manual_seed(0 if seed is None else int(seed))
             uniforms = torch.rand(B, Nmax, generator=g, device=dev)
         uniforms = uniforms.to(device=dev, dtype=torch.float32)
+        if prefill_events is not None:
+            prefill_events[0].record()
         self._prefill(cond_latent, text_tokens, st)
+        if prefill_events is not None:
+            prefill_events[1].record()
         if trace_logits is not None:   # parity hook (eager mode): logits the sampler sees at every step
             trace_logits.append(st["logits"][:1].expand(B, -1).clone())
         for ch in st["chains"]:
@@ -379,9 +384,11 @@ class AREngine:
         ch["seen"][:, 0] = 2
         ch["seen"][:, w] |= (1 << bit) if bit < 31 else -(1 << 31)
 
-    def _begin_grouped(self, cond_latent, text_tokens_list, counts, Nmax, uniforms_list, seed, sp, trace_logits=None):
+    def _begin_grouped(self, cond_latent, text_tokens_list, counts, Nmax, uniforms_list, seed, sp, trace_logits=None,
+                       prefill_events=None):
         """_begin for a batch of utterances: one prefill per utterance into its own prefix, and the first token of every
-        row sampled from its utterance's prefill logits (one sampler call per chain, so the step counter advances once)."""
+        row sampled from its utterance's prefill logits (one sampler call per chain, so the step counter advances once).
+        `prefill_events`: None or a pair of CUDA events recorded around the prefills."""
         dev = self.dev
         Ps = [len(t) + 4 for t in text_tokens_list]
         st = self._decode_state(sum(counts), None, Nmax, counts, Ps)
@@ -393,8 +400,12 @@ class AREngine:
                 u = torch.rand(n, Nmax, generator=g, device=dev)
             us.append(u.to(device=dev, dtype=torch.float32))
         uniforms = torch.cat(us, dim=0)
+        if prefill_events is not None:
+            prefill_events[0].record()
         for gs, toks in zip(st["groups"], text_tokens_list):
             self._prefill(cond_latent, toks, gs)
+        if prefill_events is not None:
+            prefill_events[1].record()
         first = torch.cat([gs["logits"].expand(gs["b1"] - gs["b0"], -1) for gs in st["groups"]], dim=0)
         if trace_logits is not None:
             trace_logits.append(first.clone())
@@ -463,28 +474,31 @@ class AREngine:
 
     def generate(self, cond_latent, text_tokens, num_candidates, max_new, uniforms=None, seed=None, temperature=0.8,
                  top_k=50, top_p=0.8, repetition_penalty=2.0, pos_mode="ref_kv_quirk", use_graph=True,
-                 stop_check_every=32, trace_logits=None, typical_mass=None):
+                 stop_check_every=32, trace_logits=None, typical_mass=None, prefill_events=None):
         """≙ num_candidates/bs calls of UnifiedVoice.inference_speech (autoregressive.py:535-563), all candidates in
         ONE batch with a shared-prefix KV cache. Returns int32 codes [num_candidates, max_new] padded with the
         stop token (api.py:425-426). `uniforms` [B, max_new] injects the sampling randomness (parity mode).
         `typical_mass` (in (0, 1]) turns on the reference's typical-set filter (TypicalLogitsWarper after the repetition
-        penalty, autoregressive.py:558); None leaves it off."""
+        penalty, autoregressive.py:558); None leaves it off. `prefill_events`: None or a pair of CUDA events recorded
+        around the prompt prefill."""
         B, Nmax = int(num_candidates), int(max_new)
         sp = self._sampling(temperature, top_k, top_p, repetition_penalty, pos_mode, typical_mass)
         if trace_logits is not None:
             use_graph = False
-        st = self._begin(cond_latent, text_tokens, B, Nmax, uniforms, seed, sp, trace_logits)
+        st = self._begin(cond_latent, text_tokens, B, Nmax, uniforms, seed, sp, trace_logits, prefill_events)
         self._decode(st, sp, Nmax - 1, use_graph, stop_check_every, trace_logits)
         return self._codes(st)
 
     def generate_grouped(self, cond_latent, text_tokens_list, counts, max_new, uniforms_list=None, seed=None,
                          temperature=0.8, top_k=50, top_p=0.8, repetition_penalty=2.0, pos_mode="ref_kv_quirk",
-                         use_graph=True, stop_check_every=32, trace_logits=None, typical_mass=None):
+                         use_graph=True, stop_check_every=32, trace_logits=None, typical_mass=None,
+                         prefill_events=None):
         """Several utterances decoded in ONE batch: utterance u contributes counts[u] candidates that attend to its own
         prompt (text_tokens_list[u], one shared conditioning latent). Returns one int32 codes tensor [counts[u], max_new]
         per utterance, each as generate(cond_latent, text_tokens_list[u], counts[u], max_new, uniforms_list[u], ...)
         returns it. At most lib.AR_STEP_MAX_GROUPS utterances, lib.AR_STEP_MAX_B rows and prompts of
-        lib.AR_STEP_MAX_P positions (plan_batches packs within these limits); the one-kernel step is required."""
+        lib.AR_STEP_MAX_P positions (plan_batches packs within these limits); the one-kernel step is required.
+        `prefill_events`: None or a pair of CUDA events recorded around the prefills."""
         counts = [int(n) for n in counts]
         if len(counts) != len(text_tokens_list) or (uniforms_list is not None and len(uniforms_list) != len(counts)):
             raise ValueError("one entry of counts (and of uniforms_list) per utterance")
@@ -492,7 +506,8 @@ class AREngine:
         sp = self._sampling(temperature, top_k, top_p, repetition_penalty, pos_mode, typical_mass)
         if trace_logits is not None:
             use_graph = False
-        st = self._begin_grouped(cond_latent, text_tokens_list, counts, Nmax, uniforms_list, seed, sp, trace_logits)
+        st = self._begin_grouped(cond_latent, text_tokens_list, counts, Nmax, uniforms_list, seed, sp, trace_logits,
+                                 prefill_events)
         self._decode(st, sp, Nmax - 1, use_graph, stop_check_every, trace_logits)
         codes = self._codes(st)
         return [codes[g["b0"]: g["b1"]].clone() for g in st["groups"]]

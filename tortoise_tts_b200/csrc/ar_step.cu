@@ -46,7 +46,7 @@ constexpr int AS_MAX_TILES = 512;                          // ticket counters (r
 constexpr int AS_SYNC_BAR_BYTES = 17 * 128;                // barrier epoch line + 16 arrival-counter lines
 constexpr int AS_COMPACT_WARPS = 8;                        // ar_attn_compact_kernel: 256 threads, ~118 KB at P = 174
 constexpr int AS_COMPACT_CTAS = 2;                         // ar_attn_compact_kernel CTAs per SM
-constexpr int AS_MAX_GROUPS = 16;                          // prompt-prefix groups of one step (TtbArStepArgs.groups)
+constexpr int AS_MAX_GROUPS = 256;                         // prompt-prefix groups of one step (TtbArStepArgs.groups): one per row
 
 enum { G_QKV = 0, G_PROJ = 1, G_FC = 2, G_PROJ2 = 3, G_HEAD = 4 };
 enum { OUT_PARTIAL = 0, OUT_BF16 = 1, OUT_F32 = 2 };
@@ -61,7 +61,8 @@ struct AsLayer {       // device table, one per layer
 
 // One prompt-prefix group of the attention phase: rows [b0, next b0) attend to a prefix of P positions (tensor map
 // maps[4 L + 6 + g]); its attention units are [u0, next u0), ncph CTAs per head. Entry [groups] is a sentinel whose
-// b0 is B and whose u0 is the total number of units.
+// b0 is B and whose u0 is the total number of units. The table ([groups + 1] entries, up to 4 KB) lives in the device
+// tables behind the layer table, not in the kernel parameters.
 struct AsGroup {
   int b0, P, u0, ncph;
 };
@@ -70,11 +71,13 @@ struct AsParams {
   int B, D, H, L, V, Nmax, pos_mode;
   int TB, nbt, nst, stage_bytes;          // batch tile (wgmma N), number of batch tiles, pipeline stages
   int units, ipr, team;                   // attention: work units (group, head, chunk), items per round, warps per item
-  AsGroup gtab[AS_MAX_GROUPS + 1];        // [groups + 1] (one group when every row shares one prompt)
+  int ngroups;                            // prompt groups (1 when every row shares one prompt)
+  int P0, ncph0;                          // prompt positions and CTAs per head of the batch when ngroups = 1
   int layer_begin, layer_end, phase_mask; // debug / profiling: subset of the step (phase_mask bit i = phase i of a layer)
   AsGemmShape g[5];
   const CUtensorMap* maps;                // device: [4*L + 1] weight maps, then activation maps a, o, h, hn
   const AsLayer* layers;                  // device: [L]
+  const AsGroup* gtab;                    // device: [ngroups + 1], behind the layer table
   const float *lnf_g, *lnf_b, *fn_g, *fn_b, *b_head;
   const float *mel_emb, *mel_pos;
   const int* codes;
@@ -509,12 +512,22 @@ TTB_DEVINL void attn_phase_mma(const AsParams& p, int layer, uint8_t* data, Ctrl
   __nv_bfloat16* ckv_l = p.cand_kv + (long long)layer * B * H * Nmax * 128;
   int g = 0;
   for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
-    while (u >= p.gtab[g + 1].u0) ++g;                   // a CTA's units only grow: its group only advances
-    const int gb0 = p.gtab[g].b0, gB = p.gtab[g + 1].b0 - gb0, ncph = p.gtab[g].ncph;
-    const int P = p.gtab[g].P;
+    // the unit's group: the last g with u0 <= u, by bisection over [g, ngroups) (a CTA's units only grow, so its group
+    // only advances). One group (every tts() call): the values come from the parameters; reading the table here cost
+    // ~2 % of the one-row decode of 603 tokens on H100
+    int gb0 = 0, gB = B, ncph = p.ncph0, P = p.P0, lu = u;
+    if (p.ngroups > 1) {
+      for (int hi = p.ngroups; hi - g > 1;) {
+        const int mid = (g + hi) >> 1;
+        if (__ldg(&p.gtab[mid].u0) <= u) g = mid; else hi = mid;
+      }
+      const AsGroup* ge = p.gtab + g;
+      gb0 = __ldg(&ge->b0); gB = __ldg(&ge[1].b0) - gb0; ncph = __ldg(&ge->ncph);
+      P = __ldg(&ge->P);
+      lu = u - __ldg(&ge->u0);
+    }
     const CUtensorMap* map_p = map_c + 1 + g;            // prompt prefix of this unit's group
     const int npc = (P + 15) / 16;
-    const int lu = u - p.gtab[g].u0;
     const int h = lu % H, ci = lu / H;
     const int b_begin = gb0 + (int)((long long)ci * gB / ncph), b_end = gb0 + (int)((long long)(ci + 1) * gB / ncph);
     __syncthreads();
@@ -893,6 +906,7 @@ __global__ void ar_step_store_prefix_kernel(const __nv_bfloat16* __restrict__ qk
 // ------------------------------------------------------------------ host: plan
 struct AsPlan {
   AsParams p;
+  AsGroup gtab[AS_MAX_GROUPS + 1];        // host copy of the group table (ttb_ar_step_setup writes it to the device)
   long long part_floats;
   int grid;
   int ngroups;                            // >= 1 (groups == 0 is one group of every row)
@@ -926,11 +940,13 @@ static void plan_gemm(AsGemmShape& g, int Nrows, int K, int nbt, int grid, int c
 static int make_plan(const TtbArStepArgs& a, AsPlan& pl) {
   AsParams& p = pl.p;
   memset(&p, 0, sizeof(p));
+  memset(pl.gtab, 0, sizeof(pl.gtab));
   if (a.B <= 0 || a.B > 256) { set_error("ttb_ar_step: B=%d unsupported (1..256)", a.B); return -1; }
   if (a.D != a.H * 64 || a.D % 128 != 0 || a.D > 1024) { set_error("ttb_ar_step: D=%d H=%d unsupported (D = 64 H, D %% 128 == 0, D <= 1024)", a.D, a.H); return -1; }
   if (a.groups < 0 || a.groups > AS_MAX_GROUPS) { set_error("ttb_ar_step: %d prompt groups (0..%d)", a.groups, AS_MAX_GROUPS); return -1; }
   // prompt groups: rows [group_begin[g], group_begin[g + 1]) share the prefix group_prefix_kv[g] of group_P[g] positions
   pl.ngroups = a.groups > 0 ? a.groups : 1;
+  p.ngroups = pl.ngroups;
   if (a.groups > 0) {
     if (!a.group_begin || !a.group_P || !a.group_prefix_kv) { set_error("ttb_ar_step: missing group arrays"); return -1; }
     if (a.group_begin[0] != 0 || a.group_begin[a.groups] != a.B) {
@@ -939,15 +955,15 @@ static int make_plan(const TtbArStepArgs& a, AsPlan& pl) {
     for (int g = 0; g < a.groups; ++g) {
       if (a.group_begin[g + 1] <= a.group_begin[g]) { set_error("ttb_ar_step: group %d has no rows", g); return -1; }
       if (!a.group_prefix_kv[g]) { set_error("ttb_ar_step: group %d has no prefix", g); return -1; }
-      p.gtab[g].b0 = a.group_begin[g]; p.gtab[g].P = a.group_P[g];
+      pl.gtab[g].b0 = a.group_begin[g]; pl.gtab[g].P = a.group_P[g];
     }
   } else {
-    p.gtab[0].b0 = 0; p.gtab[0].P = a.P;
+    pl.gtab[0].b0 = 0; pl.gtab[0].P = a.P;
   }
-  p.gtab[pl.ngroups].b0 = a.B;
+  pl.gtab[pl.ngroups].b0 = a.B;
   int maxP = 0;
   for (int g = 0; g < pl.ngroups; ++g) {
-    const int P = p.gtab[g].P;
+    const int P = pl.gtab[g].P;
     if (P <= 0 || P > AS_MAX_P) { set_error("ttb_ar_step: prompt length P=%d exceeds %d", P, AS_MAX_P); return -1; }
     if (P > maxP) maxP = P;
   }
@@ -982,8 +998,8 @@ static int make_plan(const TtbArStepArgs& a, AsPlan& pl) {
   int max_items = 1;
   p.units = 0;
   for (int g = 0; g < pl.ngroups; ++g) {
-    AsGroup& gr = p.gtab[g];
-    const int gB = p.gtab[g + 1].b0 - gr.b0;
+    AsGroup& gr = pl.gtab[g];
+    const int gB = pl.gtab[g + 1].b0 - gr.b0;
     gr.ncph = (int)((long long)ncph * gB / a.B);
     if (gr.ncph < 1) gr.ncph = 1;
     if (gr.ncph > gB) gr.ncph = gB;
@@ -992,7 +1008,8 @@ static int make_plan(const TtbArStepArgs& a, AsPlan& pl) {
     const int items = (gB + gr.ncph - 1) / gr.ncph;
     if (items > max_items) max_items = items;
   }
-  p.gtab[pl.ngroups].u0 = p.units;
+  pl.gtab[pl.ngroups].u0 = p.units;
+  p.P0 = pl.gtab[0].P; p.ncph0 = pl.gtab[0].ncph;
   const int wcap = a.attn_compact ? AS_COMPACT_WARPS : AS_WARPS;
   const int rounds = (max_items + wcap - 1) / wcap;
   p.ipr = (max_items + rounds - 1) / rounds;
@@ -1019,10 +1036,13 @@ static int make_plan(const TtbArStepArgs& a, AsPlan& pl) {
 }
 
 constexpr int AS_EXTRA_MAPS = 6;      // activations a, o, h, hn; candidate KV cache; prompt-prefix KV cache of group 0
-// device tables: tensor maps (weights, extra maps, the prefixes of groups 1..), layer table
+// device tables: tensor maps (weights, extra maps, the prefixes of groups 1..), layer table, group table
 static int num_maps(int L, int ngroups) { return 4 * L + 1 + AS_EXTRA_MAPS + (ngroups - 1); }
+static size_t group_table_offset(int L, int ngroups) {
+  return (size_t)num_maps(L, ngroups) * sizeof(CUtensorMap) + (size_t)L * sizeof(AsLayer);
+}
 static long long table_bytes(int L, int ngroups) {
-  return (long long)num_maps(L, ngroups) * sizeof(CUtensorMap) + (long long)L * sizeof(AsLayer) + 256;
+  return (long long)group_table_offset(L, ngroups) + (long long)(ngroups + 1) * sizeof(AsGroup) + 256;
 }
 
 }  // namespace ttb
@@ -1050,6 +1070,7 @@ extern "C" int ttb_ar_step_setup(const TtbArStepArgs* ap, void* stream) {
   std::vector<unsigned char> host((size_t)table_bytes(a.L, pl.ngroups), 0);
   CUtensorMap* maps = reinterpret_cast<CUtensorMap*>(host.data());
   AsLayer* lay = reinterpret_cast<AsLayer*>(host.data() + (size_t)nmaps * sizeof(CUtensorMap));
+  memcpy(host.data() + group_table_offset(a.L, pl.ngroups), pl.gtab, (size_t)(pl.ngroups + 1) * sizeof(AsGroup));
   const uint64_t D = a.D;
   for (int l = 0; l < a.L; ++l) {
     const TtbArStepLayer& s = a.layers[l];
@@ -1076,7 +1097,7 @@ extern "C" int ttb_ar_step_setup(const TtbArStepArgs* ap, void* stream) {
     if (make_tensor_map_bf16_nd(&am[4], a.cand_kv, 4, cd, cs, box)) return -1;
     // prompt prefix of group g, [L][H][P_g][2][64]: maps[4 L + 6 + g]
     for (int g = 0; g < pl.ngroups; ++g) {
-      const uint64_t P = (uint64_t)pl.p.gtab[g].P;
+      const uint64_t P = (uint64_t)pl.gtab[g].P;
       const uint64_t pd[4] = {64, 2, P, (uint64_t)a.L * a.H};
       const uint64_t ps[3] = {128, 256, P * 256};
       const void* pkv = a.groups > 0 ? a.group_prefix_kv[g] : a.prefix_kv;
@@ -1107,6 +1128,7 @@ extern "C" int ttb_ar_decode_step(const TtbArStepArgs* ap, void* stream) {
   const int nmaps = num_maps(a.L, pl.ngroups);
   p.maps = reinterpret_cast<const CUtensorMap*>(a.tables);
   p.layers = reinterpret_cast<const AsLayer*>(reinterpret_cast<const unsigned char*>(a.tables) + (size_t)nmaps * sizeof(CUtensorMap));
+  p.gtab = reinterpret_cast<const AsGroup*>(reinterpret_cast<const unsigned char*>(a.tables) + group_table_offset(a.L, pl.ngroups));
   p.lnf_g = a.lnf_g; p.lnf_b = a.lnf_b; p.fn_g = a.fn_g; p.fn_b = a.fn_b; p.b_head = a.b_head;
   p.mel_emb = a.mel_emb; p.mel_pos = a.mel_pos; p.codes = a.codes; p.ld_codes = a.ld_codes; p.state = a.state;
   p.x = a.x;

@@ -230,7 +230,7 @@ def ar_step_store_prefix(qkv, P, H, pkv):
 
 
 AR_STEP_MAX_B, AR_STEP_MAX_P, AR_STEP_MAX_D = 256, 352, 1024    # limits of csrc/ar_step.cu (make_plan)
-AR_STEP_MAX_GROUPS = 16                                          # prompt groups of one step (TtbArStepArgs.groups)
+AR_STEP_MAX_GROUPS = 256                                         # prompt groups of one step (TtbArStepArgs.groups)
 
 
 def ar_step_supported(B, D, H, P):
