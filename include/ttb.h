@@ -267,6 +267,13 @@ typedef struct TtbDiffStepArgs {
  * learned-range variance, eps->x0 clamp, posterior mean, ancestral noise; denormalize_tacotron_mel on the
  * last step (utils/audio.py:63-64). */
 int ttb_diffusion_step(const TtbDiffStepArgs* args, void* stream);
+/* ddim_sample epilogue (utils/diffusion.py:623-671) on the same arguments, with another meaning of `tables`:
+ * fp32 [5, iters] rows sqrt_recip_ac, sqrt_recipm1_ac, sqrt(ac_prev), dir = sqrt(1 - ac_prev - sigma^2), sigma
+ * (diffusion_engine.make_ddim_schedule). Per element: the same CFG mix, x0 = clamp(sqrt_recip_ac*x - sqrt_recipm1_ac*eps,
+ * -1, 1), eps re-derived from the clamped x0, x' = sqrt(ac_prev)*x0 + dir*eps + sigma*noise (no noise at i == 0); the
+ * learned-variance half of model_out is not read. `noise` may be NULL when every sigma is 0 (eta = 0). x_bf16, mel_out
+ * and parity_stride act as in the p_sample epilogue above. */
+int ttb_ddim_step(const TtbDiffStepArgs* args, void* stream);
 /* CFG branch pair on two GPUs (no reference counterpart: the reference runs both branches on one device,
  * utils/diffusion.py:340-342): copies this rank's branch output `src` (n floats) into slot (call & 1, branch_off) of the
  * local AND the partner's exchange area (peer memory mapped through CUDA IPC), publishes epoch + call + 1 in the

@@ -162,6 +162,20 @@ def _typical_mass(typical_sampling, typical_mass):
     return m
 
 
+DIFFUSION_SAMPLERS = ("p", "ddim")
+
+
+def _sampler_kwargs(diffusion_sampler, ddim_eta):
+    """DiffusionEngine.sample kwargs for the tts() kwargs `diffusion_sampler` / `ddim_eta`. An unknown sampler or an eta
+    outside [0, 1] raises ValueError. The default sampler adds no kwargs, so its call is exactly the p-sampler call."""
+    if diffusion_sampler not in DIFFUSION_SAMPLERS:
+        raise ValueError("diffusion_sampler must be one of %s, got %r" % (DIFFUSION_SAMPLERS, diffusion_sampler))
+    eta = float(ddim_eta)
+    if not 0.0 <= eta <= 1.0:
+        raise ValueError("ddim_eta must lie in [0, 1], got %r" % (ddim_eta,))
+    return {} if diffusion_sampler == "p" else {"sampler": diffusion_sampler, "eta": eta}
+
+
 _CLASSIFIERS = {}
 
 
@@ -440,7 +454,7 @@ class TextToSpeech:
                    use_deterministic_seed=None, num_autoregressive_samples=512, temperature=.8, length_penalty=1,
                    repetition_penalty=2.0, top_p=.8, max_mel_tokens=500, cvvp_amount=.0, diffusion_iterations=100,
                    cond_free=True, cond_free_k=2, diffusion_temperature=1.0, top_k=50, typical_sampling=False,
-                   typical_mass=.9, **hf_generate_kwargs):
+                   typical_mass=.9, diffusion_sampler="p", ddim_eta=0.0, **hf_generate_kwargs):
         from .text import utterance_plan
         from .ar_engine import plan_batches
         if hf_generate_kwargs:
@@ -449,6 +463,7 @@ class TextToSpeech:
         if ws > 1 and k != 1:
             raise NotImplementedError("tts_batch on several ranks renders one waveform per text: k must be 1")
         typical = _typical_mass(typical_sampling, typical_mass)
+        sampler_kw = _sampler_kwargs(diffusion_sampler, ddim_eta)
         seed = self.deterministic_state(seed=use_deterministic_seed)
         auto_cond, diff_cond, auto_conds, _ = self._conditioning(voice_samples, conditioning_latents)
         plan = utterance_plan(len(texts), ws)
@@ -484,7 +499,7 @@ class TextToSpeech:
                     e = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
                     res, t = self._render(texts[u], toks[u], c, B, k, seed, auto_cond, diff_cond, auto_conds,
                                           cvvp_amount, diffusion_iterations, cond_free, cond_free_k,
-                                          diffusion_temperature, e)
+                                          diffusion_temperature, e, sampler_kw)
                     parts[u] = res if len(res) > 1 else res[0]
                     t["clvp_ms"] = e[0].elapsed_time(e[1])
                     for key, v in t.items():
@@ -503,13 +518,17 @@ class TextToSpeech:
             return_deterministic_state=False, num_autoregressive_samples=512, temperature=.8, length_penalty=1,
             repetition_penalty=2.0, top_p=.8, max_mel_tokens=500, cvvp_amount=.0, diffusion_iterations=100,
             cond_free=True, cond_free_k=2, diffusion_temperature=1.0, text_tokens=None, top_k=50, typical_sampling=False,
-            typical_mass=.9, **hf_generate_kwargs):
+            typical_mass=.9, diffusion_sampler="p", ddim_eta=0.0, **hf_generate_kwargs):
         """≙ TextToSpeech.tts (api.py:334-597). `text_tokens` (list of BPE ids) may be given instead of `text`.
         `typical_sampling` / `typical_mass` are the reference's generate kwargs of the same names (api.py:361-364): the
-        sampler keeps only the typical set of mass `typical_mass` (in (0, 1]) of the penalised scores."""
+        sampler keeps only the typical set of mass `typical_mass` (in (0, 1]) of the penalised scores.
+        `diffusion_sampler` picks the diffusion decoder's sampler on the same respaced schedule: "p" (the reference's
+        p_sample_loop, the default) or "ddim" (its ddim_sample_loop, utils/diffusion.py:711-793) with `ddim_eta` in [0, 1]
+        (0: deterministic given x_T). Both draw the same noises from the same seed, so they start from the same x_T."""
         if hf_generate_kwargs:
             raise TypeError(f"unsupported generate kwargs: {sorted(hf_generate_kwargs)}")
         typical = _typical_mass(typical_sampling, typical_mass)
+        sampler_kw = _sampler_kwargs(diffusion_sampler, ddim_eta)
         seed = self.deterministic_state(seed=use_deterministic_seed)
         auto_cond, diff_cond, auto_conds, conditioning_latents = self._conditioning(voice_samples, conditioning_latents)
         toks = self._text_ids(text, text_tokens)
@@ -531,7 +550,8 @@ class TextToSpeech:
                                                  pos_mode="ref_kv_quirk" if self.kv_cache else "train_consistent",
                                                  typical_mass=typical)
             res, t = self._render(text, toks, codes, B, k, seed, auto_cond, diff_cond, auto_conds, cvvp_amount,
-                                  diffusion_iterations, cond_free, cond_free_k, diffusion_temperature, ev[1:4])
+                                  diffusion_iterations, cond_free, cond_free_k, diffusion_temperature, ev[1:4],
+                                  sampler_kw)
             self.last_timings = {"ar_ms": ev[0].elapsed_time(ev[1]), "clvp_ms": ev[1].elapsed_time(ev[2]), **t,
                                  "device_total_ms": ev[0].elapsed_time(ev[3])}
         out = res if len(res) > 1 else res[0]
@@ -563,11 +583,12 @@ class TextToSpeech:
         return toks
 
     def _render(self, text, toks, codes, B, k, seed, auto_cond, diff_cond, auto_conds, cvvp_amount, diffusion_iterations,
-                cond_free, cond_free_k, diffusion_temperature, ev):
+                cond_free, cond_free_k, diffusion_temperature, ev, sampler_kw):
         """What tts() does after the decode, for one utterance: fix the codes of this rank's candidates, rank all B
         candidates (CLVP / CVVP, top-k), then latents, calm-token trim, diffusion, vocoder and redaction of the k best.
-        Records ev[0] after the fix, ev[1] after the ranking, ev[2] after the rendering. Returns (list of k waveforms
-        [1, 1, S] on the CPU, {stage: device ms} of the rendering stages)."""
+        Records ev[0] after the fix, ev[1] after the ranking, ev[2] after the rendering. `sampler_kw` (from
+        _sampler_kwargs) goes to DiffusionEngine.sample. Returns (list of k waveforms [1, 1, S] on the CPU, {stage:
+        device ms} of the rendering stages)."""
         dev = self.device
         rank, ws = parallel.world()
         with torch.no_grad():
@@ -618,7 +639,7 @@ class TextToSpeech:
                 owner, p = plan[j]
                 pair = None if p is None else (groups[p], rank - owner)
                 mel = self.diffusion.sample(lat, diff_cond, diffusion_iterations, noise0, step_noise, cond_free=cond_free,
-                                            cond_free_k=cond_free_k, pair=pair)
+                                            cond_free_k=cond_free_k, pair=pair, **sampler_kw)
                 e[2].record()
                 if self.debug_capture:
                     self.last_debug["latents"][j] = lat.clone()

@@ -178,6 +178,40 @@ diffusion_step_kernel(TtbDiffStepArgs a) {
   }
 }
 
+// DDIM step epilogue (eq. 12 of Song et al.). One thread per (s, c). The learned-variance half of model_out is not read.
+__global__ void __launch_bounds__(256)
+ddim_step_kernel(TtbDiffStepArgs a) {
+  const long long idx = (long long)blockIdx.x * 256 + threadIdx.x;
+  if (idx >= (long long)a.S * a.C) return;
+  const int s = (int)(idx / a.C), c = (int)(idx - (long long)s * a.C);
+  const int call = *a.step;
+  const int i = a.iters - 1 - call;
+  const float* tb = a.tables;
+  const float sra = tb[0 * a.iters + i], srm1 = tb[1 * a.iters + i], sab_prev = tb[2 * a.iters + i],
+              dir = tb[3 * a.iters + i], sigma = tb[4 * a.iters + i];
+  const float* mob = a.model_out + (long long)(call & 1) * a.parity_stride;
+  float eps = mob[(long long)s * a.ld_out + c];
+  if (a.cond_free) {
+    const float eps_u = mob[a.out_bstride + (long long)s * a.ld_out + c];
+    const double cfkd = (double)a.cond_free_k * (1.0 - (double)i / (double)a.iters);
+    eps = (float)(1.0 + cfkd) * eps - (float)cfkd * eps_u;
+  }
+  const float xt = a.x[idx];
+  const float sx = sra * xt;
+  const float x0 = fminf(fmaxf(sx - srm1 * eps, -1.0f), 1.0f);
+  // eps re-derived from the clamped x0 (_predict_eps_from_xstart), not the model's eps
+  const float eps_x0 = (sx - x0) / srm1;
+  const float nz = (i == 0) ? 0.f : 1.f;
+  const float noise = a.noise ? a.noise[(long long)call * a.S * a.C + idx] : 0.f;
+  const float xn = (sab_prev * x0 + dir * eps_x0) + nz * sigma * noise;
+  a.x[idx] = xn;
+  if (a.x_bf16) reinterpret_cast<__nv_bfloat16*>(a.x_bf16)[(long long)s * a.ld_xb + c] = __float2bfloat16(xn);
+  if (a.mel_out && i == 0) {
+    const float MX = 2.3143386840820312f, MN = -11.512925148010254f;
+    a.mel_out[(long long)c * a.S + s] = ((xn + 1.0f) / 2.0f) * (MX - MN) + MN;
+  }
+}
+
 __global__ void counter_add_kernel(int* c, int d) { *c += d; }
 
 // ------------------------------------------------------------------ CFG pair: exchange of the two denoiser branches
@@ -291,6 +325,12 @@ extern "C" int ttb_diffusion_step(const TtbDiffStepArgs* args, void* stream) {
   const long long n = (long long)args->S * args->C;
   diffusion_step_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ST>>>(*args);
   TTB_CHECK_LAUNCH("diffusion_step_kernel");
+  return 0;
+}
+extern "C" int ttb_ddim_step(const TtbDiffStepArgs* args, void* stream) {
+  const long long n = (long long)args->S * args->C;
+  ddim_step_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ST>>>(*args);
+  TTB_CHECK_LAUNCH("ddim_step_kernel");
   return 0;
 }
 extern "C" int ttb_pair_exchange(const float* src, float* local_area, float* peer_area, long long n, long long parity_stride,

@@ -1,8 +1,9 @@
 """DiffusionTts denoiser + SpacedDiffusion sampling loop on the sm_90a kernels (hot loop 2, SURVEY §8 rows a9-a12).
 
 Mirrors `do_spectrogram_diffusion` (tortoise/api.py:117-130): `timestep_independent` once, then `iters` steps of
-p_sample with the conditional and unconditional forward batched as B=2 (the reference runs them sequentially,
-utils/diffusion.py:340-342), scheduler tables resident on the device and the whole step captured in one CUDA graph.
+p_sample (or ddim_sample with `sample(sampler="ddim")`) with the conditional and unconditional forward batched as B=2
+(the reference runs them sequentially, utils/diffusion.py:340-342), scheduler tables resident on the device and the
+whole step captured in one CUDA graph.
 Activations are token-major [B, S, C]; convolutions are wgmma GEMMs (k=3 as three shifted TMA loads).
 """
 import math
@@ -35,9 +36,8 @@ def _groups_for(C):
 
 
 # ----------------------------------------------------------------------- schedule (host, float64 like the reference)
-def make_schedule(iters, trained_steps=4000):
-    """SpacedDiffusion(space_timesteps(4000,[iters]), linear betas) tables (utils/diffusion.py:94-111,1093-1115,
-    1184-1205,192-249). Returns (timestep_map int64[n], tables float32 [6, n])."""
+def _respace(iters, trained_steps):
+    """-> (timestep_map int64 [n], betas float64 [n]) of SpacedDiffusion(space_timesteps(trained_steps, [iters]))."""
     scale = 1000 / trained_steps
     base_betas = np.linspace(scale * 0.0001, scale * 0.02, trained_steps, dtype=np.float64)
     base_ac = np.cumprod(1.0 - base_betas, axis=0)
@@ -52,7 +52,13 @@ def make_schedule(iters, trained_steps=4000):
             betas.append(1 - ac / last)
             last = ac
             tmap.append(i)
-    betas = np.array(betas, dtype=np.float64)
+    return np.array(tmap, dtype=np.int64), np.array(betas, dtype=np.float64)
+
+
+def make_schedule(iters, trained_steps=4000):
+    """SpacedDiffusion(space_timesteps(4000,[iters]), linear betas) tables (utils/diffusion.py:94-111,1093-1115,
+    1184-1205,192-249). Returns (timestep_map int64[n], tables float32 [6, n])."""
+    tmap, betas = _respace(iters, trained_steps)
     alphas = 1.0 - betas
     ac = np.cumprod(alphas, axis=0)
     ac_prev = np.append(1.0, ac[:-1])
@@ -60,7 +66,23 @@ def make_schedule(iters, trained_steps=4000):
     tables = np.stack([
         np.sqrt(1.0 / ac), np.sqrt(1.0 / ac - 1), np.log(np.append(post_var[1], post_var[1:])), np.log(betas),
         betas * np.sqrt(ac_prev) / (1.0 - ac), (1.0 - ac_prev) * np.sqrt(alphas) / (1.0 - ac)]).astype(np.float32)
-    return np.array(tmap, dtype=np.int64), tables
+    return tmap, tables
+
+
+def make_ddim_schedule(iters, eta, trained_steps=4000):
+    """The tables of ddim_sample (utils/diffusion.py:623-671) on the schedule of make_schedule, built in float64.
+    Returns (timestep_map int64 [n], tables float32 [5, n]): sqrt_recip_ac, sqrt_recipm1_ac, sqrt(ac_prev),
+    dir = sqrt(max(0, 1 - ac_prev - sigma^2)) and sigma = eta sqrt((1 - ac_prev) / (1 - ac)) sqrt(1 - ac / ac_prev).
+    The reference takes the square roots of dir and sigma in fp32 torch; here they are taken in float64 and rounded once,
+    so the tables differ from its values by fp32 rounding, and dir's radicand (exactly 0 at the last step) cannot be
+    rounded below 0 at eta = 1."""
+    tmap, betas = _respace(iters, trained_steps)
+    ac = np.cumprod(1.0 - betas, axis=0)
+    ac_prev = np.append(1.0, ac[:-1])
+    sigma = eta * np.sqrt((1.0 - ac_prev) / (1.0 - ac)) * np.sqrt(1.0 - ac / ac_prev)
+    tables = np.stack([np.sqrt(1.0 / ac), np.sqrt(1.0 / ac - 1), np.sqrt(ac_prev),
+                       np.sqrt(np.maximum(0.0, 1.0 - ac_prev - sigma ** 2)), sigma]).astype(np.float32)
+    return tmap, tables
 
 
 def _rel_pos_table(emb_weight, T, scale):
@@ -269,6 +291,7 @@ class DiffusionEngine:
         self._epilogue(st)
 
     def _epilogue(self, st):
+        step = lib.ddim_step if st["sampler"] == "ddim" else lib.diffusion_step
         xch = st.get("xch")
         if xch is not None:
             # CFG pair over peer memory: one captured launch puts my branch into both exchange areas and waits for the
@@ -276,9 +299,8 @@ class DiffusionEngine:
             n = st["S"] * self.cout
             lib.pair_exchange(st["mo_local"], xch.area, xch.peer_area, n, 2 * n, xch.my_idx * n, xch.peer_flags, xch.flags,
                               st["counter"], xch.epoch, xch.done, xch.err)
-            lib.diffusion_step(xch.area, n, self.cout, st["x"], st["x_bf"], self.cin_pad, st["noise"], st["tables"],
-                               st["counter"], st["S"], self.cin, st["iters"], st["cond_free"], st["cond_free_k"], st["mel"],
-                               parity_stride=2 * n)
+            step(xch.area, n, self.cout, st["x"], st["x_bf"], self.cin_pad, st["noise"], st["tables"], st["counter"],
+                 st["S"], self.cin, st["iters"], st["cond_free"], st["cond_free_k"], st["mel"], parity_stride=2 * n)
             lib.counter_add(st["counter"], 1)
             return
         if st.get("pair") is not None:
@@ -290,19 +312,20 @@ class DiffusionEngine:
                 dist.all_gather_into_tensor(st["model_out"].view(-1), st["mo_local"].view(-1), group=st["pair"][0])
             else:   # gloo (CPU tests of the host logic)
                 dist.all_gather([st["model_out"][0], st["model_out"][1]], st["mo_local"][0], group=st["pair"][0])
-        lib.diffusion_step(st["model_out"], st["S"] * self.cout, self.cout, st["x"], st["x_bf"], self.cin_pad, st["noise"],
-                           st["tables"], st["counter"], st["S"], self.cin, st["iters"], st["cond_free"],
-                           st["cond_free_k"], st["mel"])
+        step(st["model_out"], st["S"] * self.cout, self.cout, st["x"], st["x_bf"], self.cin_pad, st["noise"], st["tables"],
+             st["counter"], st["S"], self.cin, st["iters"], st["cond_free"], st["cond_free_k"], st["mel"])
         lib.counter_add(st["counter"], 1)
 
-    def _state(self, S, B, iters, cfk=0.0, pair=None):
-        """B = number of CFG branches evaluated ON THIS RANK (2, or 1 when the pair is split over two GPUs / no CFG)."""
-        key = (S, B, iters, cfk, None if pair is None else pair[1])
+    def _state(self, S, B, iters, cfk=0.0, pair=None, sampler="p"):
+        """B = number of CFG branches evaluated ON THIS RANK (2, or 1 when the pair is split over two GPUs / no CFG).
+        The captured graph holds the sampler's epilogue, so the sampler is part of the key; DDIM's eta lives only in
+        st['tables']."""
+        key = (S, B, iters, cfk, None if pair is None else pair[1], sampler)
         if self._ws is not None and self._ws["key"] == key:
             self._ws["pair"] = pair
             return self._ws
         C, dev = self.C, self.dev
-        st = dict(key=key, S=S, B=B, iters=iters, pair=pair)
+        st = dict(key=key, S=S, B=B, iters=iters, pair=pair, sampler=sampler)
         st["ws"] = self._alloc(B, S)
         st["xce"] = torch.empty(B, S, C, dtype=torch.float32, device=dev)
         st["code_emb_init"] = torch.empty(B, S, C, dtype=torch.float32, device=dev)
@@ -360,9 +383,11 @@ class DiffusionEngine:
         return mo[0].t().contiguous(), mo[1].t().contiguous()
 
     def sample(self, latents, cond_latent, iters, noise0, step_noise, cond_free=True, cond_free_k=2.0, use_graph=True,
-               return_trace=False, pair=None):
+               return_trace=False, pair=None, sampler="p", eta=0.0):
         """≙ do_spectrogram_diffusion (api.py:117-130). latents [N, ar_dim], cond_latent [2C];
         noise0 [100, S] (already scaled by the temperature), step_noise [iters, 100, S] in call order.
+        `sampler`: "p" runs p_sample_loop, "ddim" runs ddim_sample_loop with `eta` in [0, 1] (utils/diffusion.py:711-793)
+        on the same respaced schedule and model call; DDIM reads step_noise[c] at call c too, scaled by sigma.
         Returns the denormalised mel fp32 [100, S] (channel-major, as the reference returns it)."""
         C, dev = self.C, self.dev
         N = latents.shape[0]
@@ -371,9 +396,16 @@ class DiffusionEngine:
         if not cond_free:
             pair = None
         B = 1 if (pair is not None or not cond_free) else 2
-        tmap, tables = make_schedule(iters)
+        if sampler == "p":
+            tmap, tables = make_schedule(iters)
+        elif sampler == "ddim":
+            if not 0.0 <= eta <= 1.0:
+                raise ValueError("ddim eta must lie in [0, 1], got %r" % (eta,))
+            tmap, tables = make_ddim_schedule(iters, float(eta))
+        else:
+            raise ValueError("unknown diffusion sampler %r (expected 'p' or 'ddim')" % (sampler,))
         n = len(tmap)
-        st = self._state(S, B, n, float(cond_free_k), pair)
+        st = self._state(S, B, n, float(cond_free_k), pair, sampler)
         st["cond_free"], st["cond_free_k"] = bool(cond_free), float(cond_free_k)
         if pair is None or pair[1] == 0:
             code_emb = self.timestep_independent(latents, cond_latent, S)
@@ -382,7 +414,7 @@ class DiffusionEngine:
             lib.broadcast_rows(self.uncond, S, C, st["code_emb_init"][0], None, C)
         if B == 2:
             lib.broadcast_rows(self.uncond, S, C, st["code_emb_init"][1], None, C)
-        st["tables"].copy_(torch.from_numpy(tables))
+        st["tables"][:tables.shape[0]].copy_(torch.from_numpy(tables))
         # time embeddings of all steps in call order (i = n-1 ... 0), then every ResBlock's emb_layers
         self._prepare_time(st, [int(tmap[n - 1 - c]) for c in range(n)])
         # state: x_T and the pre-drawn noises, token-major
