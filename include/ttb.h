@@ -175,6 +175,16 @@ int ttb_ar_sample_typical(const float* logits, int ld_logits, int V, int B, cons
                           uint32_t* seen, int* codes, int ld_codes, int* finished, TtbArState* state, float temperature,
                           int top_k, float top_p, float rep_penalty, int stop_token, int advance, float typical_mass,
                           void* stream);
+/* The latent the reference's streaming generator yields next to each token (stream_generator.py:982,
+ * final_norm(hidden_states[-1][:, -1]) of the step that sampled it), taken from the decode step itself: for every row b,
+ * out[b * ld_row + j * D + c] = final_norm(ln_f(x[b, :]))[c] with j = state->step - 1. x fp32 [B, D] is the residual
+ * stream a decode step leaves behind (ttb_ar_decode_step, or ttb_residual_layernorm before the final norms), and the call
+ * is enqueued AFTER the sampler of that step: ttb_ar_sample advances state->step, so step - 1 is the index of the token
+ * the step just sampled (nothing is written when it lies outside [0, Nmax)). Same arithmetic as
+ * ttb_layernorm(x, ..., out_f32): the result equals it bit for bit. D a multiple of 128, <= 1024; ld_row >= Nmax * D
+ * (fp32 elements, a multiple of 4); 16-byte aligned pointers. CUDA-graph capturable. */
+int ttb_ar_capture_latents(const float* x, int B, int D, const float* g1, const float* b1, const float* g2,
+                           const float* b2, const TtbArState* state, int Nmax, float* out, long long ld_row, void* stream);
 /* fix_autoregressive_output (api.py:87-114) for every row + calm-token trim length (api.py:547-556) */
 int ttb_ar_fix_codes(int* codes, int B, int L, int stop_token, int* trim_len, void* stream);
 /* rows of an embedding table + optional positional table -> fp32 [n, D]; ids int32, pos int32 (or NULL) */

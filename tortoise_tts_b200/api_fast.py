@@ -4,7 +4,8 @@ directly by the HiFiGAN decoder (`hifidecoder.pth`), optionally streamed chunk b
 
 Same constructor, `tts()`, `tts_stream()`, `tts_with_preset()`, `handle_chunks()`, `get_conditioning_latents()`
 (auto latent only, api_fast.py:225-246), `get_random_conditioning_latents()` (api_fast.py:248-254) and
-`deterministic_state()`. Everything between the tokenizer and the returned waveform runs in libttb.so: the decode
+`deterministic_state()`. Beyond the reference: `tts_batch()` / `tts_long()` (many sentences in one decode batch) and
+their streaming forms `tts_stream_batch()` / `tts_long_stream()`. Everything between the tokenizer and the returned waveform runs in libttb.so: the decode
 loop (`AREngine.generate` / `generate_stream`), the latent pass (`AREngine.latents` / `stream_latents`) and the
 decoder (`HifiganEngine`).
 
@@ -40,6 +41,17 @@ PRESETS = {  # api_fast.py:265-270
 _DIFFUSION_ONLY = ("diffusion_iterations", "cond_free", "cond_free_k", "diffusion_temperature")
 STREAM_MAX_LENGTH = 500      # autoregressive.py:571: prompt + generated tokens of the streaming generator
 FIRST_BUFFER = 60            # api_fast.py:398
+
+
+def stream_flushes(n, flushed, ended, stream_chunk_size):
+    """The flush rule of the streaming mode (api_fast.py:393-419), for one stream: `n` tokens have arrived, the previous
+    flush covered `flushed` of them (0: none yet), `ended` says whether the stream is over. Returns the flushes due now,
+    in order, as a list of `is_end` flags: one flush when the tokens buffered since the last flush reach the threshold
+    (max(stream_chunk_size, 60) before the first flush, stream_chunk_size after it; never when stream_chunk_size <= 0),
+    and one more when the stream has ended, even if nothing arrived since the last flush."""
+    every = int(stream_chunk_size)
+    due = every > 0 and (n - flushed) >= (max(every, FIRST_BUFFER) if flushed == 0 else every)
+    return ([False] if due else []) + ([True] if ended else [])
 
 
 def get_model_path(model_name, models_dir=MODELS_DIR):
@@ -198,10 +210,7 @@ class TextToSpeech:
                     temperature=temperature, top_k=top_k, top_p=top_p, repetition_penalty=repetition_penalty,
                     pos_mode=pos, use_graph=self.device.type == "cuda"):
                 n = int(codes.numel())
-                # the reference flushes when the tokens buffered since the last flush reach the threshold, and once more
-                # when the generator is exhausted (even if nothing new arrived since the last flush)
-                due = flush_every > 0 and (n - flushed) >= (first if flushed == 0 else flush_every)
-                for is_end in ([False] if due else []) + ([True] if ended else []):
+                for is_end in stream_flushes(n, flushed, ended, flush_every):
                     lat = self.autoregressive.stream_latents(auto, toks, codes) if pos == "ref_kv_quirk" else \
                         self._stream_latents_train(auto, toks, codes)
                     wav_gen = self.hifi_decoder.inference(lat, auto)
@@ -271,7 +280,7 @@ class TextToSpeech:
         return wav.reshape(1, 1, -1), n
 
     # ------------------------------------------------------------------ several sentences per call
-    def tts_batch(self, texts, voice_samples=None, text_tokens_list=None, **kwargs):
+    def tts_batch(self, texts, voice_samples=None, text_tokens_list=None, conditioning_latents_list=None, **kwargs):
         """Several sentences in one call, each ONE sequence: entry u of the returned list is what
         `tts(texts[u], voice_samples, **kwargs)` returns (fp32 [1, 1, samples] on the device). The conditioning latent
         and the seed are computed once, and every sentence samples with the uniforms row tts() draws from that seed.
@@ -279,18 +288,37 @@ class TextToSpeech:
         one row per sentence, each attending to its own prompt (ar_engine.plan_batches), so a batch costs about one
         decode step per token instead of one per sentence and token. A sentence whose prompt is longer than 352
         positions is decoded alone, as tts() decodes it. The stop-token cut, the latent pass and HiFiGAN then run per
-        sentence as in tts(). `text_tokens_list` (one id list per text) bypasses the tokenizer. `last_timings`: ar_ms
+        sentence as in tts(). `text_tokens_list` (one id list per text) bypasses the tokenizer.
+        `conditioning_latents_list`: one auto conditioning latent per text (as get_conditioning_latents returns it), so
+        that one batch holds several voices; with get_conditioning_latents(clips) as entry u, entry u of the result is
+        tts(texts[u], voice_samples=clips). It excludes `voice_samples`. `last_timings`: ar_ms
         (the decode batches, prefills included), prefill_ms (their prompt prefills), latents_ms and hifigan_ms (summed
         over the sentences), device_total_ms, and tokens (the tokens kept per sentence). Every rank computes the whole
         batch, as tts() does."""
         texts = list(texts)
         if not texts:
             raise ValueError("tts_batch needs at least one text")
+        self._check_lists(texts, voice_samples, text_tokens_list, conditioning_latents_list)
+        return self._tts_batch(texts, voice_samples, text_tokens_list, conditioning_latents_list, **kwargs)
+
+    @staticmethod
+    def _check_lists(texts, voice_samples, text_tokens_list, conditioning_latents_list):
         if text_tokens_list is not None and len(text_tokens_list) != len(texts):
             raise ValueError("text_tokens_list has %d entries for %d texts" % (len(text_tokens_list), len(texts)))
-        return self._tts_batch(texts, voice_samples, text_tokens_list, **kwargs)
+        if conditioning_latents_list is not None:
+            if voice_samples is not None:
+                raise ValueError("give voice_samples (one voice for every text) or conditioning_latents_list, not both")
+            if len(conditioning_latents_list) != len(texts):
+                raise ValueError("conditioning_latents_list has %d entries for %d texts" %
+                                 (len(conditioning_latents_list), len(texts)))
 
-    def _tts_batch(self, texts, voice_samples, text_tokens_list, k=1, verbose=True, use_deterministic_seed=None,
+    def _auto_latents(self, n, voice_samples, conditioning_latents_list):
+        """The auto conditioning latent of each of n texts: conditioning_latents_list, else one voice for all."""
+        if conditioning_latents_list is not None:
+            return [c.to(self.device).float().reshape(-1) for c in conditioning_latents_list]
+        return [self._auto_latent(voice_samples)] * n
+
+    def _tts_batch(self, texts, voice_samples, text_tokens_list, conditioning_latents_list, k=1, verbose=True, use_deterministic_seed=None,
                    num_autoregressive_samples=512, temperature=.8, length_penalty=1, repetition_penalty=2.0, top_p=.8,
                    max_mel_tokens=500, cvvp_amount=.0, top_k=50, typical_sampling=False, typical_mass=.9,
                    **hf_generate_kwargs):
@@ -301,7 +329,7 @@ class TextToSpeech:
         seed = self.deterministic_state(seed=use_deterministic_seed)
         toks = [self._inputs_tokens(texts[u], None if text_tokens_list is None else text_tokens_list[u])
                 for u in range(len(texts))]
-        auto = self._auto_latent(voice_samples)
+        autos = self._auto_latents(len(texts), voice_samples, conditioning_latents_list)
         if verbose:
             print("Generating autoregressive samples..")
         n_max = self.cfg.max_mel_tokens - 1
@@ -327,16 +355,17 @@ class TextToSpeech:
                 if timed:
                     ev[0].record()
                 if len(batch) == 1:
-                    codes = [ar.generate(auto, toks[batch[0]], 1, n_max, uniforms=uniforms, prefill_events=pre, **dec)]
+                    codes = [ar.generate(autos[batch[0]], toks[batch[0]], 1, n_max, uniforms=uniforms,
+                                         prefill_events=pre, **dec)]
                 else:
-                    codes = ar.generate_grouped(auto, [toks[u] for u in batch], [1] * len(batch), n_max,
-                                                uniforms_list=[uniforms] * len(batch), prefill_events=pre, **dec)
+                    codes = ar.generate_grouped([autos[u] for u in batch], [toks[u] for u in batch], [1] * len(batch),
+                                                n_max, uniforms_list=[uniforms] * len(batch), prefill_events=pre, **dec)
                 if timed:
                     ev[3].record()
                     timed_parts.append((ev, [("ar_ms", 0, 3), ("prefill_ms", 1, 2)]))
                 for u, c in zip(batch, codes):
                     e = new_events(3)
-                    wavs[u], tokens[u] = self._render(auto, toks[u], c, n_max, False,
+                    wavs[u], tokens[u] = self._render(autos[u], toks[u], c, n_max, False,
                                                       (lambda i, e=e: e[i].record()) if timed else None, 0)
                     if timed:
                         timed_parts.append((e, [("latents_ms", 0, 1), ("hifigan_ms", 1, 2)]))
@@ -362,3 +391,158 @@ class TextToSpeech:
             raise ValueError("text_tokens_list has %d entries for %d chunks" % (len(text_tokens_list), len(texts)))
         wavs = self.tts_batch(texts, text_tokens_list=text_tokens_list, **kwargs)
         return torch.cat([w.reshape(1, -1).cpu() for w in wavs], dim=-1)
+
+    # ------------------------------------------------------------------ many streams per call
+    def tts_stream_batch(self, texts, voice_samples=None, conditioning_latents_list=None, text_tokens_list=None,
+                         **kwargs):
+        """Streams several texts at once: a generator of `(u, chunk, last)`. For each u, the chunks arrive in the order
+        `tts_stream(texts[u], ...)` yields them, with the same count and lengths; `last` marks the final chunk of stream
+        u. Chunks of different streams interleave. Every text is one row of ONE grouped decode batch (at most
+        lib.AR_STEP_MAX_GROUPS texts, each prompt at most lib.AR_STEP_MAX_P positions; beyond that ValueError, since a
+        stream cannot wait for another batch), so the batch costs about one decode step per token for all streams.
+        Each row keeps tts_stream's flush rule (stream_flushes) and chunk state. The latents come from the decode steps
+        themselves (AREngine.generate_grouped_stream) instead of a teacher-forced pass per flush, and the rows that
+        flush at the same token count are decoded by one HifiganEngine.inference_batch call. The captured latents
+        differ from tts_stream's recomputed ones in the last bits, so the tokens are identical and the waveforms agree
+        within rounding (DESIGN §5).
+        One seed for all rows: row u samples with the uniforms tts_stream draws from it for texts[u].
+        `voice_samples`: one voice for all texts; `conditioning_latents_list`: one auto conditioning latent per text (as
+        get_conditioning_latents returns it), not both. `text_tokens_list` (one id list per text) bypasses the
+        tokenizer. The other keyword arguments are those of tts_stream, accepted and rejected as it does.
+        `last_timings` (set when the generator is exhausted): ar_ms (decode, prefills included), hifigan_ms,
+        device_total_ms and tokens (per row)."""
+        texts = list(texts)
+        if not texts:
+            raise ValueError("tts_stream_batch needs at least one text")
+        if len(texts) > lib.AR_STEP_MAX_GROUPS:
+            raise ValueError("tts_stream_batch streams at most %d texts at once, got %d" %
+                             (lib.AR_STEP_MAX_GROUPS, len(texts)))
+        self._check_lists(texts, voice_samples, text_tokens_list, conditioning_latents_list)
+        toks = [self._inputs_tokens(texts[u], None if text_tokens_list is None else text_tokens_list[u])
+                for u in range(len(texts))]
+        for u, t in enumerate(toks):
+            if len(t) + 4 > lib.AR_STEP_MAX_P:
+                raise ValueError("text %d: a prompt of %d positions (at most %d in a batch; tts_stream streams it alone)"
+                                 % (u, len(t) + 4, lib.AR_STEP_MAX_P))
+        return self._stream_batch(toks, voice_samples, conditioning_latents_list, **kwargs)
+
+    def _stream_batch(self, toks, voice_samples, conditioning_latents_list, conditioning_latents=None, k=1,
+                      verbose=True, use_deterministic_seed=None, return_deterministic_state=False, overlap_wav_len=1024,
+                      stream_chunk_size=40, num_autoregressive_samples=512, temperature=.8, length_penalty=1,
+                      repetition_penalty=2.0, top_p=.8, max_mel_tokens=500, cvvp_amount=.0, diffusion_iterations=100,
+                      cond_free=True, cond_free_k=2, diffusion_temperature=1.0, top_k=50, **hf_generate_kwargs):
+        """tts_stream's keyword arguments, checked before the generator starts."""
+        if hf_generate_kwargs:
+            raise TypeError(f"unsupported generate kwargs: {sorted(hf_generate_kwargs)}")
+        dec = dict(temperature=temperature, top_k=top_k, top_p=top_p, repetition_penalty=repetition_penalty)
+        return self._stream_batch_run(toks, voice_samples, conditioning_latents_list, verbose, use_deterministic_seed,
+                                      overlap_wav_len, int(stream_chunk_size), dec)
+
+    def _stream_batch_run(self, toks, voice_samples, conditioning_latents_list, verbose, use_deterministic_seed,
+                          overlap_wav_len, flush_every, dec):
+        R = len(toks)
+        seed = self.deterministic_state(seed=use_deterministic_seed)
+        autos = self._auto_latents(R, voice_samples, conditioning_latents_list)
+        if verbose:
+            print("Generating autoregressive samples..")
+        caps = [STREAM_MAX_LENGTH - (len(t) + 4) for t in toks]
+        if flush_every > 0:
+            first, block = max(flush_every, FIRST_BUFFER), flush_every
+        else:
+            first = block = max(caps)
+        timed = self.device.type == "cuda"
+        new_event = (lambda: torch.cuda.Event(enable_timing=True)) if timed else (lambda: None)
+        record = (lambda e: e.record()) if timed else (lambda e: None)
+        ar_parts, hifi_parts = [], []
+        wav_prev, wav_tail, flushed = [None] * R, [None] * R, [0] * R
+        done, tokens = [False] * R, [0] * R
+        with torch.no_grad():
+            start = new_event()
+            record(start)
+            # as tts_stream: each row draws its own table from the seed (a Philox draw depends on the tensor's size)
+            us = [self._uniforms(seed, c) for c in caps]
+            steps = iter(self.autoregressive.generate_grouped_stream(
+                autos, toks, caps, first, block, uniforms_list=us, pos_mode=self._pos_mode(), use_graph=timed, **dec))
+            while True:
+                e0, e1 = new_event(), new_event()
+                record(e0)
+                try:
+                    codes, ended, lat = next(steps)
+                except StopIteration:
+                    break
+                record(e1)
+                ar_parts.append((e0, e1))
+                jobs = {}                                  # token count -> [(row, flushes)]
+                for u in range(R):
+                    if done[u]:
+                        continue
+                    n = int(codes[u].numel())
+                    flags = stream_flushes(n, flushed[u], ended[u], flush_every)
+                    if flags:
+                        jobs.setdefault(n, []).append((u, flags))
+                    if ended[u]:
+                        done[u], tokens[u] = True, n
+                for n in sorted(jobs):
+                    rows = [u for u, _ in jobs[n]]
+                    h0, h1 = new_event(), new_event()
+                    record(h0)
+                    wavs = self.hifi_decoder.inference_batch(lat[rows, :n], torch.stack([autos[u] for u in rows]))
+                    record(h1)
+                    hifi_parts.append((h0, h1))
+                    for (u, flags), wav_gen in zip(jobs[n], wavs):
+                        for i, is_end in enumerate(flags):
+                            # tts_stream decodes every flush into a buffer of its own, and handle_chunks fades in place
+                            w = wav_gen if i == 0 else wav_gen.clone()
+                            chunk, wav_prev[u], wav_tail[u] = self.handle_chunks(w, wav_prev[u], wav_tail[u],
+                                                                                 overlap_wav_len)
+                            flushed[u] = n
+                            yield u, chunk, is_end
+            end = new_event()
+            record(end)
+        self.last_timings = {"tokens": tokens}
+        if timed:
+            end.synchronize()
+            self.last_timings = {"ar_ms": sum(a.elapsed_time(b) for a, b in ar_parts),
+                                 "hifigan_ms": sum(a.elapsed_time(b) for a, b in hifi_parts),
+                                 "device_total_ms": start.elapsed_time(end), "tokens": tokens}
+
+    def tts_long_stream(self, text, voice_samples=None, text_tokens_list=None, **kwargs):
+        """≙ the loop of the reference's `tts_stream.py` for one voice: split the text (`'|'` forces the split points,
+        else `split_and_recombine_text`) and stream every chunk with the SAME seed, as 1-D waveform chunks in playback
+        order: all of sentence 0, then sentence 1, and so on. The sentences are streamed by tts_stream_batch, up to 256
+        per batch (consecutive batches beyond that), so later sentences decode while the first ones play; a sentence
+        whose prompt is longer than 352 positions is streamed alone by tts_stream. `text_tokens_list` (one id list per
+        chunk) bypasses the tokenizer; the other keyword arguments are those of tts_stream."""
+        from .ar_engine import plan_batches
+        from .text import split_and_recombine_text
+        texts = text.split("|") if "|" in text else split_and_recombine_text(text)
+        if text_tokens_list is not None and len(text_tokens_list) != len(texts):
+            raise ValueError("text_tokens_list has %d entries for %d chunks" % (len(text_tokens_list), len(texts)))
+        raw = [[int(t) for t in (text_tokens_list[u] if text_tokens_list is not None else self.tokenizer.encode(texts[u]))]
+               for u in range(len(texts))]
+        return self._long_stream(texts, raw, voice_samples, kwargs,
+                                 plan_batches([(1, len(t) + 5) for t in raw], max_groups=lib.AR_STEP_MAX_GROUPS))
+
+    def _long_stream(self, texts, raw, voice_samples, kwargs, batches):
+        kwargs = dict(kwargs)
+        kwargs["use_deterministic_seed"] = self.deterministic_state(seed=kwargs.get("use_deterministic_seed"))
+        for batch in batches:
+            if len(batch) == 1 and len(raw[batch[0]]) + 5 > lib.AR_STEP_MAX_P:
+                yield from self.tts_stream(texts[batch[0]], voice_samples=voice_samples, text_tokens=raw[batch[0]],
+                                           **kwargs)
+                continue
+            pending = [[] for _ in batch]              # chunks of sentences after the one playing
+            finished = [False] * len(batch)
+            cur = 0
+            for u, chunk, last in self.tts_stream_batch([texts[i] for i in batch], voice_samples=voice_samples,
+                                                        text_tokens_list=[raw[i] for i in batch], **kwargs):
+                if u == cur:
+                    yield chunk
+                else:
+                    pending[u].append(chunk)
+                finished[u] = finished[u] or last
+                while cur < len(batch) and finished[cur]:
+                    cur += 1
+                    if cur < len(batch):
+                        yield from pending[cur]
+                        pending[cur] = []

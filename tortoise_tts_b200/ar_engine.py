@@ -301,6 +301,8 @@ class AREngine:
         if st["mode"] == "fused":
             self._step_handle(st, sp["pos_mode"]).step()
             self._sample(sp, st["logits"], self.V, st)
+            if sp.get("capture"):
+                self._capture(st)
             return
         hd = self._step_handle(st, sp["pos_mode"]) if st["mode"] == "mixed" else None
         lib.ar_embed_step(st["codes"], Nmax, st["state"], self.w.mel_emb, self.w.mel_pos, B, D, sp["pos_mode"], x)
@@ -336,6 +338,15 @@ class AREngine:
                                self.w.fn_b, out_bf16=st["hn"])
         lib.gemm(st["hn"], self.w.w_head, M=B, N=self.V, K=D, bias=self.w.b_head, out_f32=st["logits"], w_static=True)
         self._sample(sp, st["logits"], self.V, st)
+        if sp.get("capture"):
+            self._capture(st)
+
+    def _capture(self, ch):
+        """Latent capture of one chain, after its sampler: row b's latent of the token just sampled goes to
+        ch["lat"][b, step - 1] (the rows of the batch's [B, Nmax, D] buffer that belong to this chain)."""
+        w = self.w
+        lib.ar_capture_latents(ch["x"], ch["B"], self.D, w.lnf_g, w.lnf_b, w.fn_g, w.fn_b, ch["state"], ch["Nmax"],
+                               ch["lat"], ch["Nmax"] * self.D)
 
     def _sample(self, sp, logits, ld_logits, ch):
         """The sampler over the logits of one chain (ld_logits = 0: row 0 for every candidate); the typical-set entry
@@ -388,8 +399,12 @@ class AREngine:
                        prefill_events=None):
         """_begin for a batch of utterances: one prefill per utterance into its own prefix, and the first token of every
         row sampled from its utterance's prefill logits (one sampler call per chain, so the step counter advances once).
+        `cond_latent`: one conditioning latent for every utterance, or a list with one per utterance.
         `prefill_events`: None or a pair of CUDA events recorded around the prefills."""
         dev = self.dev
+        conds = list(cond_latent) if isinstance(cond_latent, (list, tuple)) else [cond_latent] * len(counts)
+        if len(conds) != len(counts):
+            raise ValueError("%d conditioning latents for %d utterances" % (len(conds), len(counts)))
         Ps = [len(t) + 4 for t in text_tokens_list]
         st = self._decode_state(sum(counts), None, Nmax, counts, Ps)
         us = []
@@ -402,8 +417,8 @@ class AREngine:
         uniforms = torch.cat(us, dim=0)
         if prefill_events is not None:
             prefill_events[0].record()
-        for gs, toks in zip(st["groups"], text_tokens_list):
-            self._prefill(cond_latent, toks, gs)
+        for gs, cond, toks in zip(st["groups"], conds, text_tokens_list):
+            self._prefill(cond, toks, gs)
         if prefill_events is not None:
             prefill_events[1].record()
         first = torch.cat([gs["logits"].expand(gs["b1"] - gs["b0"], -1) for gs in st["groups"]], dim=0)
@@ -460,11 +475,15 @@ class AREngine:
         return cs[0].clone() if len(cs) == 1 else torch.cat(cs, dim=0)
 
     @staticmethod
-    def _sampling(temperature, top_k, top_p, repetition_penalty, pos_mode, typical_mass=None):
+    def _sampling(temperature, top_k, top_p, repetition_penalty, pos_mode, typical_mass=None, capture=False):
         """The sampling parameters of a decode; also the key of the captured step graph, so a change of any of them
-        (the typical mass included) captures a new graph. typical_mass None = no typical filter."""
+        (the typical mass and the latent capture included) captures a new graph. typical_mass None = no typical filter.
+        capture: every step ends with ttb_ar_capture_latents into each chain's ch["lat"]; without it the step (and its
+        graph) is what it is without this option."""
         sp = dict(temperature=float(temperature), top_k=int(top_k), top_p=float(top_p),
                   rep_penalty=float(repetition_penalty), pos_mode=1 if pos_mode == "ref_kv_quirk" else 0)
+        if capture:
+            sp["capture"] = True
         if typical_mass is not None:
             m = float(typical_mass)
             if not 0.0 < m <= 1.0:
@@ -494,7 +513,8 @@ class AREngine:
                          use_graph=True, stop_check_every=32, trace_logits=None, typical_mass=None,
                          prefill_events=None):
         """Several utterances decoded in ONE batch: utterance u contributes counts[u] candidates that attend to its own
-        prompt (text_tokens_list[u], one shared conditioning latent). Returns one int32 codes tensor [counts[u], max_new]
+        prompt (text_tokens_list[u]; `cond_latent` is one conditioning latent for all, or a list with one per utterance,
+        each utterance's latent then starting its own prompt). Returns one int32 codes tensor [counts[u], max_new]
         per utterance, each as generate(cond_latent, text_tokens_list[u], counts[u], max_new, uniforms_list[u], ...)
         returns it. At most lib.AR_STEP_MAX_GROUPS utterances, lib.AR_STEP_MAX_B rows and prompts of
         lib.AR_STEP_MAX_P positions (plan_batches packs within these limits); the one-kernel step is required.
@@ -573,6 +593,81 @@ class AREngine:
                 yield row, True
                 return
             yield row, False
+            target = have + blk
+
+    def generate_grouped_stream(self, cond_latent, text_tokens_list, max_new, first_block, block, uniforms_list=None,
+                                seed=None, temperature=0.8, top_k=50, top_p=0.8, repetition_penalty=2.0,
+                                pos_mode="ref_kv_quirk", use_graph=True, typical_mass=None):
+        """generate_stream for several utterances, ONE row each, decoded in one grouped batch (limits of
+        generate_grouped); each row attends to its own prompt text_tokens_list[u], after its own conditioning latent
+        (`cond_latent`: one for all, or a list). `max_new`: the cap of every row, or a list with one per row; the batch
+        decodes up to the largest. uniforms_list[u]: [1, >= max_new[u]] (padded here to the batch width).
+        Every step also captures the latents the streaming generator yields next to its tokens (ttb_ar_capture_latents;
+        latent 0 is the prefill's last row), so no teacher-forced pass is needed to decode them.
+        A generator of `(codes, ended, latents)`, after the first `first_block` tokens, then every `block` tokens, until
+        every row has ended: codes[u] = int32 [n_u] the tokens of row u so far, ended[u] as generate_stream decides it
+        for that row alone (its stop token, kept as the last element, or its cap reached); a row that has ended keeps
+        its last codes in later yields. `latents` fp32 [rows, max(max_new), D]: latents[u, i] belongs to codes[u][i];
+        the buffer belongs to the decode workspace and stays valid until the next decode."""
+        n = len(text_tokens_list)
+        caps = [int(m) for m in max_new] if isinstance(max_new, (list, tuple)) else [int(max_new)] * n
+        if len(caps) != n or min(caps) < 1:
+            raise ValueError("one cap >= 1 per row: %s for %d rows" % (caps, n))
+        Nmax, D = max(caps), self.D
+        us = None
+        if uniforms_list is not None:
+            if len(uniforms_list) != n:
+                raise ValueError("one uniforms table per row")
+            us = []
+            for u, c in zip(uniforms_list, caps):
+                u = u.to(device=self.dev, dtype=torch.float32).reshape(1, -1)
+                if u.shape[1] < c:
+                    raise ValueError("uniforms of %d steps for a cap of %d" % (u.shape[1], c))
+                us.append(torch.nn.functional.pad(u[:, :Nmax], (0, max(0, Nmax - u.shape[1]))))
+        sp = self._sampling(temperature, top_k, top_p, repetition_penalty, pos_mode, typical_mass, capture=True)
+        st = self._begin_grouped(cond_latent, text_tokens_list, [1] * n, Nmax, us, seed, sp)
+        if "lat" not in st:
+            st["lat"] = torch.empty(n, Nmax, D, dtype=torch.float32, device=self.dev)
+        lat = st["lat"]
+        for ch in st["chains"]:
+            ch["lat"] = lat[ch["b0"]: ch["b0"] + ch["B"]]
+        w = self.w
+        for gs in st["groups"]:          # latent 0: final norms of the prefill's last row (the start mel token)
+            lib.layernorm(gs["px"][gs["P"] - 1:], 1, D, w.lnf_g, w.lnf_b, w.fn_g, w.fn_b, out_f32=lat[gs["b0"], 0])
+        if use_graph and Nmax > 1:
+            self._ensure_graph(st, sp)
+        stop = self.cfg.stop_mel_token
+        have = 1
+        target = max(1, int(first_block))
+        blk = max(1, int(block))
+        ended, out = [False] * n, [None] * n
+        while True:
+            # a row's blocks end where generate_stream would end them: at its own cap
+            want = min(target, max(c for c, e in zip(caps, ended) if not e))
+            for _ in range(want - have):
+                if use_graph:
+                    st["graph"].replay()
+                else:
+                    self._decode_step(st, sp)
+            if use_graph and want > have:
+                lib.add_calls((want - have) * st["graph_calls"])
+            have = max(have, want)
+            codes = self._codes(st)[:, :have]
+            if st["fused"] and have > 1:
+                self._check_step_flag(st)
+            host = codes.cpu()
+            for u in range(n):
+                if ended[u]:
+                    continue
+                m = min(have, caps[u])
+                hit = (host[u, :m] == stop).nonzero()
+                if hit.numel() > 0:
+                    out[u], ended[u] = codes[u, : int(hit[0].item()) + 1], True
+                else:
+                    out[u], ended[u] = codes[u, :m], m >= caps[u]
+            yield list(out), list(ended), lat
+            if all(ended):
+                return
             target = have + blk
 
     # ------------------------------------------------------------------ teacher-forced passes

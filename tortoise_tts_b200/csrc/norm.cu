@@ -77,6 +77,38 @@ layernorm_kernel(const float* x, int D, const float* __restrict__ g1, const floa
 // (the two block_sum round trips of the block-per-row kernel above dominate a 4 KB row). Same arithmetic as layernorm_kernel (two-pass variance, fixed
 // summation order of the split-K partials), only the reduction tree differs.
 
+// The LayerNorm(s) of one warp's row, in place: v[i] holds columns (i * 32 + lane) * 4 .. + 3. g2 == nullptr: one LN.
+template <int NV>
+TTB_DEVINL void ln_warp_row(float4 (&v)[NV], int lane, int D, const float* __restrict__ g1, const float* __restrict__ b1,
+                            const float* __restrict__ g2, const float* __restrict__ b2) {
+#pragma unroll
+  for (int pass = 0; pass < 2; ++pass) {
+    const float* gg = pass == 0 ? g1 : g2;
+    const float* bb = pass == 0 ? b1 : b2;
+    if (!gg) break;
+    float s = 0.f;
+#pragma unroll
+    for (int i = 0; i < NV; ++i) s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
+    const float mean = warp_sum(s) / D;
+    float q = 0.f;
+#pragma unroll
+    for (int i = 0; i < NV; ++i) {
+      const float dx = v[i].x - mean, dy = v[i].y - mean, dz = v[i].z - mean, dw = v[i].w - mean;
+      q += (dx * dx + dy * dy) + (dz * dz + dw * dw);
+    }
+    const float rstd = rsqrtf(warp_sum(q) / D + 1e-5f);
+#pragma unroll
+    for (int i = 0; i < NV; ++i) {
+      const float4 ga = *reinterpret_cast<const float4*>(gg + (i * 32 + lane) * 4);
+      const float4 be = *reinterpret_cast<const float4*>(bb + (i * 32 + lane) * 4);
+      v[i].x = (v[i].x - mean) * rstd * ga.x + be.x;
+      v[i].y = (v[i].y - mean) * rstd * ga.y + be.y;
+      v[i].z = (v[i].z - mean) * rstd * ga.z + be.z;
+      v[i].w = (v[i].w - mean) * rstd * ga.w + be.w;
+    }
+  }
+}
+
 template <int NV>
 __global__ void __launch_bounds__(64)
 layernorm_warp_kernel(const float* x, int M, int D, const float* __restrict__ g1, const float* __restrict__ b1,
@@ -115,38 +147,35 @@ layernorm_warp_kernel(const float* x, int M, int D, const float* __restrict__ g1
       *reinterpret_cast<float4*>(xw + row * D + (i * 32 + lane) * 4) = v[i];
     }
   }
-#pragma unroll
-  for (int pass = 0; pass < 2; ++pass) {
-    const float* gg = pass == 0 ? g1 : g2;
-    const float* bb = pass == 0 ? b1 : b2;
-    if (!gg) break;
-    float s = 0.f;
-#pragma unroll
-    for (int i = 0; i < NV; ++i) s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
-    const float mean = warp_sum(s) / D;
-    float q = 0.f;
-#pragma unroll
-    for (int i = 0; i < NV; ++i) {
-      const float dx = v[i].x - mean, dy = v[i].y - mean, dz = v[i].z - mean, dw = v[i].w - mean;
-      q += (dx * dx + dy * dy) + (dz * dz + dw * dw);
-    }
-    const float rstd = rsqrtf(warp_sum(q) / D + 1e-5f);
-#pragma unroll
-    for (int i = 0; i < NV; ++i) {
-      const float4 ga = *reinterpret_cast<const float4*>(gg + (i * 32 + lane) * 4);
-      const float4 be = *reinterpret_cast<const float4*>(bb + (i * 32 + lane) * 4);
-      v[i].x = (v[i].x - mean) * rstd * ga.x + be.x;
-      v[i].y = (v[i].y - mean) * rstd * ga.y + be.y;
-      v[i].z = (v[i].z - mean) * rstd * ga.z + be.z;
-      v[i].w = (v[i].w - mean) * rstd * ga.w + be.w;
-    }
-  }
+  ln_warp_row<NV>(v, lane, D, g1, b1, g2, b2);
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
     const int c = (i * 32 + lane) * 4;
     if (ob) *reinterpret_cast<uint2*>(ob + row * D + c) = make_uint2(pack_bf16(v[i].x, v[i].y), pack_bf16(v[i].z, v[i].w));
     if (of) *reinterpret_cast<float4*>(of + row * D + c) = v[i];
   }
+}
+
+// ttb_ar_capture_latents: the latent of the token the decode step just sampled, one warp per row. The sampler has already
+// advanced the step counter, so that token is number state->step - 1. Same LayerNorm arithmetic as layernorm_warp_kernel,
+// which is what ttb_layernorm runs at these widths: a captured latent equals ttb_layernorm(x, out_f32) of the same x.
+template <int NV>
+__global__ void __launch_bounds__(64)
+ar_capture_latents_kernel(const float* __restrict__ x, int B, int D, const float* __restrict__ g1,
+                          const float* __restrict__ b1, const float* __restrict__ g2, const float* __restrict__ b2,
+                          const TtbArState* __restrict__ state, int Nmax, float* __restrict__ out, long long ld_row) {
+  const int lane = threadIdx.x & 31;
+  const long long row = (long long)blockIdx.x * 2 + (threadIdx.x >> 5);
+  const int j = state->step - 1;
+  if (row >= B || j < 0 || j >= Nmax) return;
+  const float* xr = x + row * D;
+  float4 v[NV];
+#pragma unroll
+  for (int i = 0; i < NV; ++i) v[i] = *reinterpret_cast<const float4*>(xr + (i * 32 + lane) * 4);
+  ln_warp_row<NV>(v, lane, D, g1, b1, g2, b2);
+  float* o = out + row * ld_row + (long long)j * D;
+#pragma unroll
+  for (int i = 0; i < NV; ++i) *reinterpret_cast<float4*>(o + (i * 32 + lane) * 4) = v[i];
 }
 
 template <int MAXV>
@@ -521,6 +550,31 @@ extern "C" int ttb_residual_layernorm(float* x, int M, int D, const float* parti
   else if (D <= 4096) layernorm_kernel<16><<<M, 256, 0, st>>>(x, D, g1, b1, g2, b2, ob, out_f32, x, partials, nsplit, split_stride, bias);
   else { set_error("ttb_residual_layernorm: D=%d > 4096", D); return -1; }
   TTB_CHECK_LAUNCH("layernorm_kernel(residual)");
+  return 0;
+}
+
+extern "C" int ttb_ar_capture_latents(const float* x, int B, int D, const float* g1, const float* b1, const float* g2,
+                                      const float* b2, const TtbArState* state, int Nmax, float* out, long long ld_row,
+                                      void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (B <= 0) return 0;
+  const void* ptrs[] = {x, g1, b1, g2, b2, out};
+  bool aligned = (ld_row & 3) == 0 && ld_row >= (long long)Nmax * D;
+  for (const void* p : ptrs) aligned = aligned && p && !(reinterpret_cast<uintptr_t>(p) & 15);
+  if (D % 128 != 0 || D > 1024 || Nmax <= 0 || !state || !aligned) {
+    set_error("ttb_ar_capture_latents: needs D a multiple of 128 <= 1024 (D=%d), Nmax > 0, ld_row >= Nmax * D, a multiple "
+              "of 4, and 16-byte aligned pointers", D);
+    return -1;
+  }
+  const dim3 grid((B + 1) / 2);
+#define TTB_CAP_CASE(NV)                                                                                             \
+  case NV: ar_capture_latents_kernel<NV><<<grid, 64, 0, st>>>(x, B, D, g1, b1, g2, b2, state, Nmax, out, ld_row); break;
+  switch (D / 128) {
+    TTB_CAP_CASE(1) TTB_CAP_CASE(2) TTB_CAP_CASE(3) TTB_CAP_CASE(4) TTB_CAP_CASE(5) TTB_CAP_CASE(6) TTB_CAP_CASE(7)
+    TTB_CAP_CASE(8)
+  }
+#undef TTB_CAP_CASE
+  TTB_CHECK_LAUNCH("ar_capture_latents_kernel");
   return 0;
 }
 

@@ -15,6 +15,10 @@ Everything is token-major `[T, C]` and every convolution is one wgmma GEMM (`ttb
     of the input rows q - 1, q, q + 1 (the third tap's weights are zero), and the `[T, s C_out]` result IS the token-major
     `[T s, C_out]` tensor;
   * the speaker conditioning `cond_layer(g)` is constant over time: folded into conv_pre's bias per call.
+
+`inference_batch` decodes R utterances of the same length in one pass: every convolution is one batched GEMM (each
+item zero-padded at its own edges, `rows` / `a_bstride`) that runs the kernel one item alone runs, so each item's sums
+are those of `inference`; the speaker term differs per item and enters conv_pre as a per-item residual row.
 """
 import math
 
@@ -106,12 +110,34 @@ class HifiganEngine:
         lib.act_split_cast(a, R, C, out, _kt(C), b=b, c=c, scale=scale, slope=slope)
         return out
 
-    def _conv(self, a, w, bias, T, cin, cout, k, dil=1, residual=None, out=None, act=lib.ACT_NONE):
-        out = torch.empty(T, cout, dtype=torch.float32, device=self.dev) if out is None else out
+    def _conv(self, a, w, bias, T, cin, cout, k, dil=1, residual=None, out=None, act=lib.ACT_NONE, R=1, res_rows=True):
+        """One convolution over T rows; R > 1: R items of T rows each, stacked ([R, T, .] tensors). res_rows False: the
+        residual is one row per item ([R, cout]), added to every row of that item."""
+        if out is None:
+            out = torch.empty(*((T, cout) if R == 1 else (R, T, cout)), dtype=torch.float32, device=self.dev)
         tile = 32 if cout <= 32 else (64 if cout <= 64 else 0)
+        if R == 1 and res_rows:
+            lib.gemm(a, w, M=T, N=cout, K=_kt(cin), taps=k, pad=dil * (k - 1) // 2, tap_dilation=dil, bias=bias,
+                     residual=residual, out_f32=out, act=act, tile_n=tile)
+            return out
+        # ttb_gemm picks its kernel from the whole problem; force the one a single item gets (ttb_gemm's rule for
+        # tile_n = 0: the warp-specialised 128x256 kernel from one wave of 128x128 tiles on, else 64-wide tiles)
+        variant = 0
+        if tile == 0:
+            if ((cout + 127) // 128) * ((T + 127) // 128) >= self._num_sms():
+                variant = 7
+            else:
+                tile = 64
         lib.gemm(a, w, M=T, N=cout, K=_kt(cin), taps=k, pad=dil * (k - 1) // 2, tap_dilation=dil, bias=bias,
-                 residual=residual, out_f32=out, act=act, tile_n=tile)
+                 residual=residual, out_f32=out, act=act, tile_n=tile, variant=variant, batch=R, rows=T,
+                 a_bstride=T * _kt(cin), res_bstride=(T if res_rows else 1) * cout, ldr=cout if res_rows else 0,
+                 outf_bstride=T * cout)
         return out
+
+    def _num_sms(self):
+        if self.dev.type != "cuda":
+            return 132
+        return torch.cuda.get_device_properties(self.dev).multi_processor_count
 
     def inference(self, latents, speaker):
         """latents fp32 [L, D] (GPT latents of ONE utterance), speaker fp32 [D] (auto conditioning latent)
@@ -150,3 +176,62 @@ class HifiganEngine:
         wav = torch.empty(T, 1, dtype=torch.float32, device=dev)
         self._conv(a, self.w_post, self.b_post, T, self.c_last, 1, 7, out=wav, act=lib.ACT_TANH)
         return wav.reshape(-1)
+
+    # rows x frames of one inference_batch pass: its activations take about 330 KB per output frame and item (the
+    # widest stage, ResBlocks over 256 x frames rows of 32 channels), so a pass stays near 5 GB; more items run in
+    # consecutive passes
+    BATCH_FRAMES = 16384
+
+    def inference_batch(self, latents, speakers):
+        """R utterances of the same length in one pass: latents fp32 [R, L, D], speakers fp32 [R, D] (one auto
+        conditioning latent each) -> waveforms fp32 [R, 256 * output_frames(L)]; row r equals
+        inference(latents[r], speakers[r]) bit for bit. Utterances of different lengths are not padded to one length
+        (zero latents do not decode to silence): they go through separate calls."""
+        dev, D = self.dev, self.D
+        lat = latents.to(dev).float()
+        R, L = int(lat.shape[0]), int(lat.shape[1])
+        lat = lat.reshape(R, L, D).contiguous()
+        spk = speakers.to(dev).float().reshape(R, D).contiguous()
+        T = self.output_frames(L)
+        wav = torch.empty(R, 256 * T, dtype=torch.float32, device=dev)
+        per = max(1, self.BATCH_FRAMES // max(T, 1))
+        for r0 in range(0, R, per):
+            r1 = min(R, r0 + per)
+            self._inference_items(lat[r0:r1], spk[r0:r1], wav[r0:r1])
+        return wav
+
+    def _inference_items(self, lat, spk, wav):
+        """inference() of R items at once, into wav [R, samples]."""
+        dev, D = self.dev, self.D
+        R, L = lat.shape[0], lat.shape[1]
+        T1 = int(math.floor(L * 4.0))
+        T = self.output_frames(L)
+        up1 = torch.empty(T1, D, dtype=torch.float32, device=dev)
+        up2 = torch.empty(R, T, D, dtype=torch.float32, device=dev)
+        for r in range(R):                 # the two interpolations, per item
+            lib.interp_linear(lat[r], L, D, 1.0 / 4.0, T1, up1)
+            lib.interp_linear(up1, T1, D, 22050.0 / 24000.0, T, up2[r])
+        spk_pre = torch.empty(R, self.C0, dtype=torch.float32, device=dev)
+        lib.linear_small(spk, R, D, self.w_cond, self.b_cond, self.C0, spk_pre)
+        # conv_pre + cond_layer(speaker): the per-item bias row enters as a residual (acc + row, as acc + bias)
+        o = self._conv(self._split(up2, R * T, D), self.w_pre, None, T, D, self.C0, 7, residual=spk_pre, R=R,
+                       res_rows=False)
+        a = self._split(o, R * T, self.C0, slope=HIFI_LRELU)
+        for i, (w_up, b_up, ch, u) in enumerate(self.ups):
+            co = ch // 2
+            o = self._conv(a, w_up, b_up, T, ch, u * co, 3, R=R)              # [R, T, u * co] == [R, T * u, co]
+            T *= u
+            streams = []
+            for k, convs in self.res[i]:
+                x = o
+                for m, (w1, b1, w2, b2, d) in enumerate(convs):
+                    t = self._conv(self._split(x, R * T, co, slope=HIFI_LRELU), w1, b1, T, co, co, k, dil=d, R=R)
+                    xn = torch.empty(R, T, co, dtype=torch.float32, device=dev) if m == 0 else x
+                    self._conv(self._split(t, R * T, co, slope=HIFI_LRELU), w2, b2, T, co, co, k, residual=x, out=xn,
+                               R=R)
+                    x = xn
+                streams.append(x)
+            last = i == len(self.ups) - 1
+            a = self._split(streams[0], R * T, co, slope=0.01 if last else HIFI_LRELU, b=streams[1], c=streams[2],
+                            scale=1.0 / len(streams))
+        self._conv(a, self.w_post, self.b_post, T, self.c_last, 1, 7, out=wav.view(R, T, 1), act=lib.ACT_TANH, R=R)

@@ -80,7 +80,7 @@ SYMBOLS = [
     "ttb_ar_step_workspace", "ttb_ar_step_setup", "ttb_ar_decode_step", "ttb_ar_step_store_prefix",
     "ttb_audio_resample", "ttb_audio_stft_mel", "ttb_mean_rows", "ttb_equal_linear",
     "ttb_pair_exchange", "ttb_enable_peer_access", "ttb_peer_alloc", "ttb_peer_open", "ttb_peer_close", "ttb_peer_free",
-    "ttb_wav2vec_conv0", "ttb_layernorm_act", "ttb_argmax_rows", "ttb_ar_sample_typical",
+    "ttb_wav2vec_conv0", "ttb_layernorm_act", "ttb_argmax_rows", "ttb_ar_sample_typical", "ttb_ar_capture_latents",
 ]
 
 
@@ -305,6 +305,13 @@ def ar_sample_typical(logits, ld_logits, V, B, uniforms, ld_u, seen, codes, ld_c
                                       ld_codes, _p(finished), _p(state), C.c_float(temperature), top_k, C.c_float(top_p),
                                       C.c_float(rep_penalty), stop_token, 1 if advance else 0, C.c_float(typical_mass),
                                       _stream()), "ttb_ar_sample_typical")
+
+
+def ar_capture_latents(x, B, D, g1, b1, g2, b2, state, Nmax, out, ld_row):
+    """out[b, state.step - 1] = final_norm(ln_f(x[b])) for the B rows of a decode step, enqueued after its sampler
+    (include/ttb.h ttb_ar_capture_latents); `ld_row` = fp32 elements between the rows of `out`."""
+    _chk(load().ttb_ar_capture_latents(_p(_f32(x)), B, D, _p(_f32(g1)), _p(_f32(b1)), _p(_f32(g2)), _p(_f32(b2)), _p(state),
+                                       Nmax, _p(_f32(out)), C.c_longlong(ld_row), _stream()), "ttb_ar_capture_latents")
 
 
 def ar_fix_codes(codes, B, L, stop_token, trim_len):
