@@ -152,6 +152,18 @@ typedef struct TtbArState {      /* device-resident, 64 ints */
  * train-consistent (j), 1 = reference kv-cache rule (j+1). tokens = codes[b, step-1]. */
 int ttb_ar_embed_step(const int* codes, int ld_codes, const TtbArState* state, const float* mel_emb,
                       const float* mel_pos, int B, int D, int pos_mode, float* x, void* stream);
+/* Per-row start steps (a stream pool: rows join a decode batch that is already running). row_start: device int32 [B] or
+ * NULL. Row b's own step is j_b = state->step - row_start[b]; it replaces state->step in every per-row index of the
+ * decode step: the token fed (codes[b, j_b - 1]) and its mel position, the KV slot written (j_b - 1) and the candidate
+ * positions attended, the sampler's codes and uniforms column, and the captured latent's column. NULL = 0 for every row:
+ * the result is the one the call without row_start gives, bit for bit.
+ * Idle-slot rule: the kernels CLAMP j_b, so no row ever indexes outside its rows of codes, uniforms, candidate KV or
+ * latents, however long a freed slot keeps stepping: to [1, Nmax] (ld_codes for ttb_ar_embed_step_rows) for the token
+ * fed, its position and the KV slot; to [0, min(ld_codes, ld_u) - 1] for the sampler's column; the capture writes
+ * nothing when j_b - 1 lies outside [0, Nmax). The shared counter state->step still advances once per sampler call.
+ * A clamped row computes garbage into its own last column only; the caller marks it finished and ignores it. */
+int ttb_ar_embed_step_rows(const int* codes, int ld_codes, const TtbArState* state, const int* row_start,
+                           const float* mel_emb, const float* mel_pos, int B, int D, int pos_mode, float* x, void* stream);
 /* One-query attention over [shared prefix | candidate KV] for every (candidate, head); appends the new K/V.
  * prefix_k/v: bf16 [H, P, 64]; cand_k/v: bf16 [B, H, Nmax, 64]; qkv bf16 [B, 3*H*64]. */
 int ttb_ar_decode_attention(const void* qkv, const void* prefix_k, const void* prefix_v, void* cand_k, void* cand_v,
@@ -167,6 +179,10 @@ int ttb_ar_store_prefix(const void* qkv, int P, int H, void* prefix_k, void* pre
 int ttb_ar_sample(const float* logits, int ld_logits, int V, int B, const float* uniforms, int ld_u, uint32_t* seen,
                   int* codes, int ld_codes, int* finished, TtbArState* state, float temperature, int top_k, float top_p,
                   float rep_penalty, int stop_token, int advance, void* stream);
+/* ttb_ar_sample with per-row start steps (row_start as for ttb_ar_embed_step_rows); ld_codes, ld_u > 0 */
+int ttb_ar_sample_rows(const float* logits, int ld_logits, int V, int B, const float* uniforms, int ld_u, uint32_t* seen,
+                       int* codes, int ld_codes, int* finished, TtbArState* state, float temperature, int top_k,
+                       float top_p, float rep_penalty, int stop_token, int advance, const int* row_start, void* stream);
 /* ttb_ar_sample with the reference's TypicalLogitsWarper(mass=typical_mass) (utils/typical_sampling.py:11-33) between
  * the repetition penalty and the temperature: only the typical set T of the penalised scores can be drawn (top-k keeps
  * min(top_k, |T|) tokens). typical_mass in (0, 1], else -1. Where the cumulative mass never reaches typical_mass
@@ -185,6 +201,10 @@ int ttb_ar_sample_typical(const float* logits, int ld_logits, int V, int B, cons
  * (fp32 elements, a multiple of 4); 16-byte aligned pointers. CUDA-graph capturable. */
 int ttb_ar_capture_latents(const float* x, int B, int D, const float* g1, const float* b1, const float* g2,
                            const float* b2, const TtbArState* state, int Nmax, float* out, long long ld_row, void* stream);
+/* ttb_ar_capture_latents with per-row start steps: row b writes column state->step - 1 - row_start[b] */
+int ttb_ar_capture_latents_rows(const float* x, int B, int D, const float* g1, const float* b1, const float* g2,
+                                const float* b2, const TtbArState* state, int Nmax, float* out, long long ld_row,
+                                const int* row_start, void* stream);
 /* fix_autoregressive_output (api.py:87-114) for every row + calm-token trim length (api.py:547-556) */
 int ttb_ar_fix_codes(int* codes, int B, int L, int stop_token, int* trim_len, void* stream);
 /* rows of an embedding table + optional positional table -> fp32 [n, D]; ids int32, pos int32 (or NULL) */
@@ -233,11 +253,23 @@ typedef struct TtbArStepArgs {
   const int* group_begin;                  /* [groups + 1] */
   const int* group_P;                      /* [groups] */
   const void* const* group_prefix_kv;      /* [groups] device pointers */
+  /* device int32 [B] or NULL: per-row start steps (see ttb_ar_embed_step_rows), for the token fed, its position and the
+   * attention's KV slot and candidate length. With row_start the attention reads every group's P from the device table
+   * (also for one group), so that ttb_ar_step_set_group_len takes effect. */
+  const int* row_start;
 } TtbArStepArgs;
 int ttb_ar_step_workspace(const TtbArStepArgs* args, long long* part_floats, long long* table_bytes, long long* sync_bytes);
 int ttb_ar_step_setup(const TtbArStepArgs* args, void* stream);      /* synchronous; once per (weights, workspace, B) */
 int ttb_ar_decode_step(const TtbArStepArgs* args, void* stream);     /* one launch; CUDA-graph capturable */
 int ttb_ar_step_store_prefix(const void* qkv, int P, int H, void* prefix_kv, void* stream);
+/* the same into a prefix of `cap` >= P positions per head, [L][H][cap][2][64] per layer slice (a slot's buffer sized for
+ * the longest prompt; its tensor map was built with group_P = cap) */
+int ttb_ar_step_store_prefix_cap(const void* qkv, int P, int cap, int H, void* prefix_kv, void* stream);
+/* Sets group `group`'s prompt length to P (0 < P <= the group_P of `args`, its prefix capacity) in the device group table
+ * that ttb_ar_step_setup wrote, as a kernel on `stream`: ordered with the decode steps, no new setup and no new graph
+ * capture. Positions [P, capacity) of the prefix are never attended to (they must hold finite values: zero the buffer
+ * once). Nothing else the plan derives from P changes: shared memory and the rings are sized at the capacity. */
+int ttb_ar_step_set_group_len(const TtbArStepArgs* args, int group, int P, void* stream);
 
 /* ---------------------------------------------------------------- CLVP */
 /* rotary (dim 32) on the first 32 dims of every head of q, k AND v (xtransformers.py:625-629,264-286);

@@ -5,7 +5,8 @@ directly by the HiFiGAN decoder (`hifidecoder.pth`), optionally streamed chunk b
 Same constructor, `tts()`, `tts_stream()`, `tts_with_preset()`, `handle_chunks()`, `get_conditioning_latents()`
 (auto latent only, api_fast.py:225-246), `get_random_conditioning_latents()` (api_fast.py:248-254) and
 `deterministic_state()`. Beyond the reference: `tts_batch()` / `tts_long()` (many sentences in one decode batch) and
-their streaming forms `tts_stream_batch()` / `tts_long_stream()`. Everything between the tokenizer and the returned waveform runs in libttb.so: the decode
+their streaming forms `tts_stream_batch()` / `tts_long_stream()`, and `stream_pool()` (texts that arrive while
+others stream join the running decode batch). Everything between the tokenizer and the returned waveform runs in libttb.so: the decode
 loop (`AREngine.generate` / `generate_stream`), the latent pass (`AREngine.latents` / `stream_latents`) and the
 decoder (`HifiganEngine`).
 
@@ -13,9 +14,11 @@ Deliberate differences (SURVEY App. D): sampling randomness comes from a device 
 `use_deterministic_seed`; `tts_with_preset` drops the diffusion-only preset keys instead of forwarding them to HF
 `generate` (which rejects them in the reference); the wav2vec redaction model is not loaded.
 """
+import collections
 import os
 import random
-from time import time
+import threading
+from time import perf_counter, time
 
 import torch
 
@@ -41,6 +44,7 @@ PRESETS = {  # api_fast.py:265-270
 _DIFFUSION_ONLY = ("diffusion_iterations", "cond_free", "cond_free_k", "diffusion_temperature")
 STREAM_MAX_LENGTH = 500      # autoregressive.py:571: prompt + generated tokens of the streaming generator
 FIRST_BUFFER = 60            # api_fast.py:398
+POOL_ADMIT_STEPS = 16        # StreamPool: decode steps between two looks at its queue
 
 
 def stream_flushes(n, flushed, ended, stream_chunk_size):
@@ -506,6 +510,19 @@ class TextToSpeech:
                                  "hifigan_ms": sum(a.elapsed_time(b) for a, b in hifi_parts),
                                  "device_total_ms": start.elapsed_time(end), "tokens": tokens}
 
+    def stream_pool(self, max_streams=64, overlap_wav_len=1024, stream_chunk_size=40, temperature=.8, length_penalty=1,
+                    repetition_penalty=2.0, top_p=.8, max_mel_tokens=500, cvvp_amount=.0, diffusion_iterations=100,
+                    cond_free=True, cond_free_k=2, diffusion_temperature=1.0, top_k=50, k=1, verbose=True,
+                    num_autoregressive_samples=512, return_deterministic_state=False, **hf_generate_kwargs):
+        """A StreamPool of `max_streams` (1..256) slots: texts submitted at any time stream from one running decode
+        batch. The keyword arguments are tts_stream's, accepted and rejected as it does; they apply to every stream."""
+        if hf_generate_kwargs:
+            raise TypeError(f"unsupported generate kwargs: {sorted(hf_generate_kwargs)}")
+        if not 1 <= int(max_streams) <= lib.AR_STEP_MAX_GROUPS:
+            raise ValueError("max_streams must lie in 1..%d, got %r" % (lib.AR_STEP_MAX_GROUPS, max_streams))
+        dec = dict(temperature=temperature, top_k=top_k, top_p=top_p, repetition_penalty=repetition_penalty)
+        return StreamPool(self, int(max_streams), overlap_wav_len, int(stream_chunk_size), dec)
+
     def tts_long_stream(self, text, voice_samples=None, text_tokens_list=None, **kwargs):
         """≙ the loop of the reference's `tts_stream.py` for one voice: split the text (`'|'` forces the split points,
         else `split_and_recombine_text`) and stream every chunk with the SAME seed, as 1-D waveform chunks in playback
@@ -546,3 +563,195 @@ class TextToSpeech:
                     if cur < len(batch):
                         yield from pending[cur]
                         pending[cur] = []
+
+
+class StreamPool:
+    """Continuous batching of tts_stream: texts join a decode batch that is already running, each in a free slot, and
+    leave it when they end. The chunks of stream `sid` are those of `tts_stream(text, voice_samples=...,
+    text_tokens=..., use_deterministic_seed=seed, **the pool's kwargs)`: the same tokens, chunk count and lengths,
+    `last` on the final chunk, whenever the text was submitted and whatever else runs. The latents come from the decode
+    steps (as in tts_stream_batch), so the samples agree with tts_stream's within rounding (DESIGN §5).
+
+    Each stream has its own voice and seed: its uniforms row and its conditioning crop follow the seed as in tts_stream.
+    The sampling parameters belong to the pool (they are part of its step graph). A full pool queues texts first in,
+    first out; the pool looks at its queue at least every POOL_ADMIT_STEPS (16) decode steps, so a text starts decoding
+    within 16 steps of a slot being free. `submit` may be called from any thread; every CUDA call happens on the thread
+    that iterates the pool (`poll` / `run`). Every stream applies stream_flushes to its own token count and ends at its
+    stop token (found no later than its next flush point) or at its cap of 500 - P tokens; its slot is then refilled
+    from the queue. HiFiGAN decodes the rows that flush at the same token count in one inference_batch pass.
+
+    `last_timings[sid]` (set when stream sid ends): tokens, wait_admit_s (submit to admission) and wait_first_chunk_s
+    (submit to first chunk, host clock); on the GPU also ar_ms (device time of the decode steps while it ran), prefill_ms
+    (its admission prefill) and hifigan_ms (the HiFiGAN passes it took part in)."""
+
+    def __init__(self, tts, max_streams, overlap_wav_len, flush_every, dec):
+        self.tts, self.capacity = tts, max_streams
+        self.overlap, self.flush_every = overlap_wav_len, flush_every
+        self.timed = tts.device.type == "cuda"
+        self.ws = tts.autoregressive.slot_workspace(max_streams, STREAM_MAX_LENGTH, pos_mode=tts._pos_mode(),
+                                                    use_graph=self.timed, **dec)
+        self.slots = [None] * max_streams
+        self.last_timings = {}
+        self._lock = threading.Lock()
+        self._queue = collections.deque()
+        self._next_sid = 0
+        self._closed = False
+        self._ar_pending = []                          # (start, end, streams running) of decode steps not yet read
+
+    def submit(self, text, voice_samples=None, conditioning_latent=None, text_tokens=None, use_deterministic_seed=None):
+        """Queues a text; returns its stream id. `conditioning_latent` (an auto latent as get_conditioning_latents
+        returns it) excludes `voice_samples`; neither = a random voice, as in tts_stream. A prompt longer than 352
+        positions raises ValueError (tts_stream can stream it alone)."""
+        if voice_samples is not None and conditioning_latent is not None:
+            raise ValueError("give voice_samples or conditioning_latent, not both")
+        toks = self.tts._inputs_tokens(text, text_tokens)
+        if len(toks) + 4 > lib.AR_STEP_MAX_P:
+            raise ValueError("a prompt of %d positions (a pool slot holds %d; tts_stream streams it alone)" %
+                             (len(toks) + 4, lib.AR_STEP_MAX_P))
+        with self._lock:
+            if self._closed:
+                raise RuntimeError("the stream pool is closed")
+            sid = self._next_sid
+            self._next_sid += 1
+            self._queue.append(dict(sid=sid, toks=toks, voice=voice_samples, cond=conditioning_latent,
+                                    seed=use_deterministic_seed, t_submit=perf_counter()))
+        return sid
+
+    def _event(self):
+        if not self.timed:
+            return None
+        e = torch.cuda.Event(enable_timing=True)
+        e.record()
+        return e
+
+    def _fill(self):
+        """Admits queued texts into free slots, first in, first out."""
+        for slot in range(self.capacity):
+            if self.slots[slot] is not None:
+                continue
+            with self._lock:
+                if not self._queue:
+                    return
+                rec = self._queue.popleft()
+            self._admit(slot, rec)
+
+    def _admit(self, slot, rec):
+        tts = self.tts
+        seed = tts.deterministic_state(seed=rec["seed"])
+        auto = rec["cond"].to(tts.device).float().reshape(-1) if rec["cond"] is not None else \
+            tts._auto_latent(rec["voice"])
+        P = len(rec["toks"]) + 4
+        cap = STREAM_MAX_LENGTH - P
+        every = self.flush_every
+        first = max(every, FIRST_BUFFER) if every > 0 else cap
+        e0 = self._event()
+        self.ws.admit(slot, auto, rec["toks"], tts._uniforms(seed, cap))
+        e1 = self._event()
+        rec.update(auto=auto, cap=cap, block=every if every > 0 else cap, obs=min(first, cap), flushed=0,
+                   wav_prev=None, wav_tail=None, t_admit=perf_counter(), t_first=None, prefill=(e0, e1),
+                   hifi=[], ar_ms=0.0)
+        self.slots[slot] = rec
+
+    def _read_ar(self):
+        """Adds the device time of the decode steps recorded so far to the streams they ran (after a synchronise)."""
+        for a, b, recs in self._ar_pending:
+            ms = a.elapsed_time(b)
+            for rec in recs:
+                rec["ar_ms"] += ms
+        self._ar_pending = []
+
+    def poll(self):
+        """Advances the pool to its next event: a list of (sid, chunk, last), or [] when no stream is active or
+        queued."""
+        stop = self.tts.cfg.stop_mel_token
+        ws = self.ws
+        while True:
+            self._fill()
+            active = [s for s in range(self.capacity) if self.slots[s] is not None]
+            if not active:
+                return []
+            n = min(self.slots[s]["obs"] - ws.tokens(s) for s in active)
+            n = min(n, POOL_ADMIT_STEPS)
+            if n > 0:
+                e0 = self._event()
+                ws.advance(n)
+                if self.timed:
+                    self._ar_pending.append((e0, self._event(), [self.slots[s] for s in active]))
+            due = [s for s in active if ws.tokens(s) >= self.slots[s]["obs"]]
+            if due:
+                return self._observe(due, stop)
+
+    def _observe(self, due, stop):
+        ws = self.ws
+        host = ws.codes().cpu()
+        ws.check()
+        if self.timed:
+            self._read_ar()
+        jobs, ended_slots = {}, []
+        for s in due:
+            rec = self.slots[s]
+            h = rec["obs"]
+            hit = (host[s, :h] == stop).nonzero()
+            if hit.numel() > 0:
+                n, ended = int(hit[0].item()) + 1, True
+            else:
+                n, ended = h, h >= rec["cap"]
+            flags = stream_flushes(n, rec["flushed"], ended, self.flush_every)
+            if flags:
+                jobs.setdefault(n, []).append((s, flags))
+            if ended:
+                rec["tokens"] = n
+                ended_slots.append(s)
+            else:
+                rec["obs"] = min(h + rec["block"], rec["cap"])
+        out = []
+        lat = ws.latents
+        for n in sorted(jobs):
+            rows = [s for s, _ in jobs[n]]
+            h0 = self._event()
+            wavs = self.tts.hifi_decoder.inference_batch(lat[rows, :n], torch.stack([self.slots[s]["auto"] for s in rows]))
+            h1 = self._event()
+            for (s, flags), wav_gen in zip(jobs[n], wavs):
+                rec = self.slots[s]
+                rec["hifi"].append((h0, h1))
+                for i, is_end in enumerate(flags):
+                    # tts_stream decodes every flush into a buffer of its own, and handle_chunks fades in place
+                    w = wav_gen if i == 0 else wav_gen.clone()
+                    chunk, rec["wav_prev"], rec["wav_tail"] = self.tts.handle_chunks(w, rec["wav_prev"], rec["wav_tail"],
+                                                                                      self.overlap)
+                    rec["flushed"] = n
+                    if rec["t_first"] is None:
+                        rec["t_first"] = perf_counter()
+                    out.append((rec["sid"], chunk, is_end))
+        for s in ended_slots:
+            self._finish(s)
+        return out
+
+    def _finish(self, s):
+        rec = self.slots[s]
+        self.ws.release(s)
+        self.slots[s] = None
+        t = {"tokens": rec["tokens"], "wait_admit_s": rec["t_admit"] - rec["t_submit"],
+             "wait_first_chunk_s": rec["t_first"] - rec["t_submit"]}
+        if self.timed:
+            if rec["hifi"]:
+                rec["hifi"][-1][1].synchronize()
+            t.update(ar_ms=rec["ar_ms"], prefill_ms=rec["prefill"][0].elapsed_time(rec["prefill"][1]),
+                     hifigan_ms=sum(a.elapsed_time(b) for a, b in rec["hifi"]))
+        self.last_timings[rec["sid"]] = t
+
+    def run(self):
+        """Yields (sid, chunk, last) until no stream is active or queued."""
+        while True:
+            ev = self.poll()
+            if not ev:
+                return
+            yield from ev
+
+    def close(self):
+        """Drops the queue and the decode workspace; the pool cannot be used afterwards."""
+        with self._lock:
+            self._closed = True
+            self._queue.clear()
+        self.slots = [None] * self.capacity
+        self.ws = None

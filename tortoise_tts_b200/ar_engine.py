@@ -19,6 +19,11 @@ def _f(t, dev):
     return t.to(device=dev, dtype=torch.float32).contiguous()
 
 
+def _rows(ch):
+    """The row_start keyword of the lib calls of a chain with per-row start steps (SlotWorkspace); none otherwise."""
+    return {} if ch.get("row_start") is None else {"row_start": ch["row_start"]}
+
+
 def plan_batches(utterances, max_rows=lib.AR_STEP_MAX_B, max_groups=lib.AR_STEP_MAX_GROUPS, max_P=lib.AR_STEP_MAX_P):
     """Packs utterances into consecutive decode batches for AREngine.generate_grouped. `utterances`: list of
     (candidates, prompt positions P). Returns a list of batches, each a list of utterance indices in order; an utterance
@@ -151,8 +156,10 @@ class AREngine:
         cfg, D, H, dev = self.cfg, self.D, self.H, self.dev
         ids = self._prompt_ids(text_tokens)
         P = len(ids) + 2
-        assert P == st["P"]
-        x = st["px"]
+        # a stream pool's slot (fused layout) holds prompts up to its capacity st["P"]; every other prefix is exact
+        assert P == st["P"] or (st["fused"] and P <= st["P"]), (P, st["P"])
+        cap = st["P"] if P != st["P"] else None
+        x = st["px"][:P]
         # rows 1..P-2: text, row P-1: start mel token at mel position 0, row 0: conditioning latent
         tid = torch.tensor(ids, dtype=torch.int32, device=dev)
         tpos = torch.arange(len(ids), dtype=torch.int32, device=dev)
@@ -165,7 +172,7 @@ class AREngine:
         for l, lw in enumerate(self.w.layers):
             def attn(qkv, o, l=l):
                 if st["fused"]:
-                    lib.ar_step_store_prefix(qkv, P, H, st["pkv"][l])
+                    lib.ar_step_store_prefix(qkv, P, H, st["pkv"][l], **({} if cap is None else {"cap": cap}))
                 else:
                     lib.ar_store_prefix(qkv, P, H, st["pk"][l], st["pv"][l])
                 lib.attention(qkv, o, nseq=1, T=P, H=H, ld=3 * D, ldo=D, k_off=D, v_off=2 * D, scale=0.125, causal=True)
@@ -181,6 +188,12 @@ class AREngine:
         if self._dec is not None and self._dec["key"] == key:
             return self._dec
         self._dec = None                  # release the previous workspace (KV caches) before allocating the next
+        self._dec = self._build_state(key, B, P, Nmax, group_rows, group_P)
+        return self._dec
+
+    def _build_state(self, key, B, P, Nmax, group_rows=None, group_P=None, shared_prefill=False):
+        """The decode workspace _decode_state describes, not kept in self._dec. shared_prefill: the groups share one set
+        of prefill buffers (px, pws), which holds only while their prefills are never kept past the next one."""
         dev = self.dev
         if group_rows is None:
             ok = lib.ar_step_supported(B, self.D, self.H, P)
@@ -202,6 +215,8 @@ class AREngine:
             b = 0
             for n, p in zip(group_rows, group_P):
                 gs = dict(P=p, fused=True, b0=b, b1=b + n)
+                if shared_prefill and st["groups"]:
+                    gs["px"], gs["pws"] = st["groups"][0]["px"], st["groups"][0]["pws"]
                 self._prefix_state(gs, p)
                 st["groups"].append(gs)
                 b += n
@@ -211,15 +226,15 @@ class AREngine:
         st["sides"] = [torch.cuda.Stream(device=dev) for _ in range(nch - 1)] if dev.type == "cuda" else []
         st["graph"] = None
         st["graph_params"] = None
-        self._dec = st
         return st
 
     def _prefix_state(self, st, P):
         """Prefill buffers and the prompt-prefix KV cache of one prompt of P positions, into the dict `st`."""
         cfg, D, dev = self.cfg, self.D, self.dev
         L, H = cfg.ar_layers, self.H
-        st["px"] = torch.empty(P, D, dtype=torch.float32, device=dev)
-        st["pws"] = self._alloc_trunk(P)
+        if "px" not in st:
+            st["px"] = torch.empty(P, D, dtype=torch.float32, device=dev)
+            st["pws"] = self._alloc_trunk(P)
         if st["fused"]:
             # K and V of a position adjacent: one (candidate, head) stream is one contiguous byte range (csrc/ar_step.cu)
             st["pkv"] = torch.empty(L, H, P, 2, 64, dtype=torch.bfloat16, device=dev)
@@ -272,7 +287,7 @@ class AREngine:
                             lnf_b=w.lnf_b, fn_g=w.fn_g, fn_b=w.fn_b, mel_emb=w.mel_emb, mel_pos=w.mel_pos,
                             codes=st["codes"], ld_codes=st["Nmax"], state=st["state"], x=st["x"], a=ws["a"], qkv=ws["qkv"],
                             o=ws["o"], h=ws["h"], hn=st["hn"], logits=st["logits"], prefix_kv=st["pkv"], cand_kv=st["ckv"],
-                            attn_compact=bool(st.get("compact")), groups=st.get("groups"))
+                            attn_compact=bool(st.get("compact")), groups=st.get("groups"), **_rows(st))
             st["step_handles"][pos_mode] = hd
         return hd
 
@@ -305,7 +320,8 @@ class AREngine:
                 self._capture(st)
             return
         hd = self._step_handle(st, sp["pos_mode"]) if st["mode"] == "mixed" else None
-        lib.ar_embed_step(st["codes"], Nmax, st["state"], self.w.mel_emb, self.w.mel_pos, B, D, sp["pos_mode"], x)
+        lib.ar_embed_step(st["codes"], Nmax, st["state"], self.w.mel_emb, self.w.mel_pos, B, D, sp["pos_mode"], x,
+                          **_rows(st))
         # Skinny-M decode (M = B candidates): every GEMM is weight-streaming bound, so the grid is widened with
         # 32-column tiles and, for the two GEMMs that feed the residual stream, split-K; their partial sums, bias and
         # the residual add are folded into the LayerNorm that follows (fixed summation order -> deterministic).
@@ -346,7 +362,7 @@ class AREngine:
         ch["lat"][b, step - 1] (the rows of the batch's [B, Nmax, D] buffer that belong to this chain)."""
         w = self.w
         lib.ar_capture_latents(ch["x"], ch["B"], self.D, w.lnf_g, w.lnf_b, w.fn_g, w.fn_b, ch["state"], ch["Nmax"],
-                               ch["lat"], ch["Nmax"] * self.D)
+                               ch["lat"], ch["Nmax"] * self.D, **_rows(ch))
 
     def _sample(self, sp, logits, ld_logits, ch):
         """The sampler over the logits of one chain (ld_logits = 0: row 0 for every candidate); the typical-set entry
@@ -355,8 +371,9 @@ class AREngine:
         args = (logits, ld_logits, self.V, ch["B"], ch["uniforms"], Nmax, ch["seen"], ch["codes"], Nmax, ch["finished"],
                 ch["state"], sp["temperature"], sp["top_k"], sp["top_p"], sp["rep_penalty"], self.cfg.stop_mel_token)
         if sp.get("typical_mass") is None:
-            lib.ar_sample(*args, advance=True)
+            lib.ar_sample(*args, advance=True, **_rows(ch))
         else:
+            assert ch.get("row_start") is None, "the typical sampler has no per-row start steps"
             lib.ar_sample_typical(*args, sp["typical_mass"], advance=True)
 
     def _begin(self, cond_latent, text_tokens, B, Nmax, uniforms, seed, sp, trace_logits=None, prefill_events=None):
@@ -384,16 +401,21 @@ class AREngine:
 
     def _reset_chain(self, ch, uniforms):
         """Sampler state of one chain before the first token; `uniforms` [B, Nmax] of the whole batch."""
+        ch["state"].zero_()
+        self._reset_rows(ch, slice(0, ch["B"]), uniforms[ch["b0"]: ch["b0"] + ch["B"]])
+
+    def _reset_rows(self, ch, rows, uniforms):
+        """Sampler state of rows `rows` (a slice) of one chain before their first token: uniforms [rows, Nmax], seen
+        bits {1, start_mel}, not finished, codes filled with the stop token."""
         cfg = self.cfg
         w, bit = divmod(cfg.start_mel_token, 32)
-        ch["uniforms"].copy_(uniforms[ch["b0"]: ch["b0"] + ch["B"]])
-        ch["state"].zero_()
-        ch["finished"].zero_()
-        ch["codes"].fill_(cfg.stop_mel_token)
-        ch["seen"].zero_()
+        ch["uniforms"][rows].copy_(uniforms)
+        ch["finished"][rows] = 0
+        ch["codes"][rows] = cfg.stop_mel_token
+        ch["seen"][rows] = 0
         # HF's repetition penalty sees the fake prompt ids {1, start_mel} (autoregressive.py:546-548)
-        ch["seen"][:, 0] = 2
-        ch["seen"][:, w] |= (1 << bit) if bit < 31 else -(1 << 31)
+        ch["seen"][rows, 0] = 2
+        ch["seen"][rows, w] |= (1 << bit) if bit < 31 else -(1 << 31)
 
     def _begin_grouped(self, cond_latent, text_tokens_list, counts, Nmax, uniforms_list, seed, sp, trace_logits=None,
                        prefill_events=None):
@@ -670,6 +692,12 @@ class AREngine:
                 return
             target = have + blk
 
+    def slot_workspace(self, capacity, max_new, temperature=0.8, top_k=50, top_p=0.8, repetition_penalty=2.0,
+                       pos_mode="ref_kv_quirk", use_graph=True):
+        """A decode workspace of `capacity` one-row slots that rows join and leave while it runs (SlotWorkspace)."""
+        return SlotWorkspace(self, capacity, max_new, self._sampling(temperature, top_k, top_p, repetition_penalty,
+                                                                     pos_mode, capture=True), use_graph)
+
     # ------------------------------------------------------------------ teacher-forced passes
     def _forward_sequences(self, emb_fn, nseq, T):
         """Runs the trunk over nseq sequences of T tokens (causal). emb_fn fills x [nseq*T, D]. Returns x."""
@@ -773,3 +801,118 @@ class AREngine:
         out = torch.empty(T, D, dtype=torch.float32, device=dev)
         lib.layernorm(x, T, D, self.w.lnf_g, self.w.lnf_b, self.w.fn_g, self.w.fn_b, out_f32=out)
         return out[Pm:].contiguous()
+
+
+class SlotWorkspace:
+    """Continuous batching: a grouped decode of `capacity` one-row groups (slots) whose step graph is captured once, and
+    into which a row joins whenever a slot is free. Every slot has a prompt prefix of lib.AR_STEP_MAX_P positions
+    (include/ttb.h ttb_ar_step_store_prefix_cap) and its own start step (TtbArStepArgs.row_start): a row admitted when
+    the shared step counter reads s has row_start s - 1, so it samples exactly the tokens that a decode of its own from
+    step 0 samples. Every step captures the latents (ttb_ar_capture_latents_rows). The step forms are those of the
+    grouped decode (fused up to FUSED_MAX_B rows, mixed, two chains from CHAINS_MIN_B rows); the per-op form has no
+    groups and raises. All calls enqueue on the current CUDA stream."""
+
+    def __init__(self, eng, capacity, max_new, sp, use_graph=True):
+        capacity, Nmax = int(capacity), int(max_new)
+        if not 1 <= capacity <= lib.AR_STEP_MAX_GROUPS:
+            raise ValueError("a slot workspace has 1..%d slots, got %d" % (lib.AR_STEP_MAX_GROUPS, capacity))
+        Pcap = lib.AR_STEP_MAX_P
+        if eng.MODE == "perop" or not lib.ar_step_supported(capacity, eng.D, eng.H, Pcap):
+            raise lib.TtbError("a slot workspace needs the one-kernel step (mode %s)" % eng.MODE)
+        self.eng, self.sp, self.capacity, self.Nmax, self.P_cap = eng, sp, capacity, Nmax, Pcap
+        self.use_graph = use_graph and eng.dev.type == "cuda"
+        dev, D = eng.dev, eng.D
+        st = eng._build_state(("slots", capacity, Nmax), capacity, None, Nmax, [1] * capacity, [Pcap] * capacity,
+                              shared_prefill=True)
+        for gs in st["groups"]:
+            # positions past a slot's prompt are loaded with its last chunk and weighted by 0: they must be finite
+            gs["pkv"].zero_()
+        st["row_start"] = torch.zeros(capacity, dtype=torch.int32, device=dev)
+        st["lat"] = torch.zeros(capacity, Nmax, D, dtype=torch.float32, device=dev)
+        self.where = []                       # slot -> (chain, row in the chain)
+        for ch in st["chains"]:
+            ch["row_start"] = st["row_start"][ch["b0"]: ch["b0"] + ch["B"]]
+            ch["lat"] = st["lat"][ch["b0"]: ch["b0"] + ch["B"]]
+            eng._reset_chain(ch, torch.zeros(capacity, Nmax, device=dev))
+            ch["finished"].fill_(1)           # an idle slot samples nothing
+            self.where += [(ch, r) for r in range(ch["B"])]
+        self.st = st
+        self.step = 0                         # host copy of every chain's state.step
+        self.rs = torch.zeros(capacity, dtype=torch.int32)      # host copy of row_start
+        self.live = [False] * capacity
+        self._first_state = torch.zeros(64, dtype=torch.int32, device=dev)   # scratch counter of the first token
+        for ch in st["chains"]:
+            eng._step_handle(ch, sp["pos_mode"])
+        if self.use_graph:
+            eng._ensure_graph(st, sp)
+
+    def admit(self, slot, cond_latent, text_tokens, uniforms_row):
+        """Starts a row in the free slot `slot`: prompt prefill into the slot's prefix, the slot's P in the step's group
+        table, its sampler state (as _reset_chain), latent 0, its row_start, and its first token, sampled from the
+        prefill logits with a scratch counter at 0 (the shared counter does not move). uniforms_row: [n] with
+        n <= max_new. Returns the prompt length P."""
+        eng, sp = self.eng, self.sp
+        if self.live[slot]:
+            raise ValueError("slot %d is in use" % slot)
+        P = len(text_tokens) + 4
+        if P > self.P_cap:
+            raise ValueError("a prompt of %d positions (a slot holds %d)" % (P, self.P_cap))
+        ch, r = self.where[slot]
+        gs = self.st["groups"][slot]
+        eng._prefill(cond_latent, text_tokens, gs)
+        eng._step_handle(ch, sp["pos_mode"]).set_group_len(r, P)
+        u = torch.zeros(1, self.Nmax, dtype=torch.float32, device=eng.dev)
+        n = min(int(uniforms_row.numel()), self.Nmax)
+        u[0, :n] = uniforms_row.reshape(-1)[:n].to(device=eng.dev, dtype=torch.float32)
+        eng._reset_rows(ch, slice(r, r + 1), u)
+        w = eng.w
+        lib.layernorm(gs["px"][P - 1:], 1, eng.D, w.lnf_g, w.lnf_b, w.fn_g, w.fn_b, out_f32=ch["lat"][r, 0])
+        self.rs[slot] = self.step - 1
+        self._first_state.zero_()
+        Nmax = self.Nmax
+        lib.ar_sample(gs["logits"], eng.V, eng.V, 1, ch["uniforms"][r:r + 1], Nmax, ch["seen"][r:r + 1],
+                      ch["codes"][r:r + 1], Nmax, ch["finished"][r:r + 1], self._first_state, sp["temperature"],
+                      sp["top_k"], sp["top_p"], sp["rep_penalty"], eng.cfg.stop_mel_token, advance=False)
+        self.live[slot] = True
+        return P
+
+    def release(self, slot):
+        """Frees a slot: its row stops sampling, and from the next advance on it is re-based every time so that it
+        attends to a few positions only (the kernels clamp it anyway)."""
+        ch, r = self.where[slot]
+        ch["finished"][r] = 1
+        self.live[slot] = False
+
+    def tokens(self, slot):
+        """Tokens sampled so far by the row in `slot`."""
+        return self.step - int(self.rs[slot])
+
+    def advance(self, n):
+        """n decode steps of every slot (graph replays)."""
+        eng, st = self.eng, self.st
+        for s in range(self.capacity):
+            if not self.live[s]:
+                self.rs[s] = self.step - 1
+        st["row_start"].copy_(self.rs)
+        for _ in range(int(n)):
+            if self.use_graph:
+                st["graph"].replay()
+            else:
+                eng._decode_step(st, self.sp)
+        if self.use_graph:
+            lib.add_calls(int(n) * st["graph_calls"])
+        self.step += int(n)
+
+    def check(self):
+        """Raises if a step reported a timed-out internal wait (fused step)."""
+        if self.st["fused"]:
+            self.eng._check_step_flag(self.st)
+
+    def codes(self):
+        """int32 [capacity, max_new]: row s holds the tokens of slot s at columns [0, tokens(s))."""
+        return self.eng._codes(self.st)
+
+    @property
+    def latents(self):
+        """fp32 [capacity, max_new, D]: latents[s, i] belongs to token i of slot s."""
+        return self.st["lat"]

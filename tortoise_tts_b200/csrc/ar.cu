@@ -15,10 +15,13 @@ __global__ void embed_kernel(const int* __restrict__ ids, const int* __restrict_
 }
 
 __global__ void ar_embed_step_kernel(const int* __restrict__ codes, int ld_codes, const TtbArState* __restrict__ state,
-                                     const float* __restrict__ mel_emb, const float* __restrict__ mel_pos, int D,
-                                     int pos_mode, float* __restrict__ x) {
+                                     const int* __restrict__ row_start, const float* __restrict__ mel_emb,
+                                     const float* __restrict__ mel_pos, int D, int pos_mode, float* __restrict__ x) {
   const int b = blockIdx.x;
-  const int j = state->step;                 // index of this token inside the mel segment (start token = 0)
+  // index of this token inside the mel segment (start token = 0); with row_start, the row's own step clamped to
+  // [1, ld_codes] (include/ttb.h)
+  int j = state->step;
+  if (row_start) j = min(max(j - row_start[b], 1), ld_codes);
   const int tok = codes[(long long)b * ld_codes + j - 1];
   const int pos = pos_mode ? j + 1 : j;      // autoregressive.py:147-149 (SURVEY App. D-1)
   const float* t = mel_emb + (long long)tok * D;
@@ -129,7 +132,7 @@ __global__ void __launch_bounds__(SAMP_THREADS)
 ar_sample_kernel(const float* __restrict__ logits, int ld_logits, int V, const float* __restrict__ uniforms, int ld_u,
                  uint32_t* __restrict__ seen, int* __restrict__ codes, int ld_codes, int* __restrict__ finished,
                  TtbArState* __restrict__ state, float temperature, int top_k, float top_p, float rep_penalty,
-                 int stop_token, int advance, float typical_mass) {
+                 int stop_token, int advance, float typical_mass, const int* __restrict__ row_start) {
   extern __shared__ float sval[];           // V floats: processed scores
   __shared__ int hist[256];
   __shared__ uint32_t s_prefix;
@@ -139,7 +142,10 @@ ar_sample_kernel(const float* __restrict__ logits, int ld_logits, int V, const f
   __shared__ int cand_i[SAMP_CAP];
   __shared__ int s_ncand;
   const int b = blockIdx.x;
-  const int step = state->step;
+  const int gstep = state->step;
+  // the column this row samples: the shared step, or with row_start the row's own step clamped to the rows of codes and
+  // uniforms (include/ttb.h)
+  const int step = row_start ? min(max(gstep - row_start[b], 0), min(ld_codes, ld_u) - 1) : gstep;
   const int words = (V + 31) >> 5;
   const int lane = threadIdx.x & 31;
   uint32_t* myseen = seen + (long long)b * words;
@@ -337,7 +343,7 @@ ar_sample_kernel(const float* __restrict__ logits, int ld_logits, int V, const f
       if (threadIdx.x == 0) {
         state->reserved[1] = 0;
         state->all_finished = unf ? 0 : 1;
-        state->step = step + 1;
+        state->step = gstep + 1;
       }
     }
   }
@@ -373,26 +379,33 @@ extern "C" int ttb_embed(const int* ids, const int* pos, int n, int D, const flo
   return 0;
 }
 
-extern "C" int ttb_ar_embed_step(const int* codes, int ld_codes, const TtbArState* state, const float* mel_emb,
-                                 const float* mel_pos, int B, int D, int pos_mode, float* x, void* stream) {
-  ar_embed_step_kernel<<<B, 256, 0, static_cast<cudaStream_t>(stream)>>>(codes, ld_codes, state, mel_emb, mel_pos, D,
-                                                                        pos_mode, x);
+extern "C" int ttb_ar_embed_step_rows(const int* codes, int ld_codes, const TtbArState* state, const int* row_start,
+                                      const float* mel_emb, const float* mel_pos, int B, int D, int pos_mode, float* x,
+                                      void* stream) {
+  ar_embed_step_kernel<<<B, 256, 0, static_cast<cudaStream_t>(stream)>>>(codes, ld_codes, state, row_start, mel_emb,
+                                                                        mel_pos, D, pos_mode, x);
   TTB_CHECK_LAUNCH("ar_embed_step_kernel");
   return 0;
+}
+
+extern "C" int ttb_ar_embed_step(const int* codes, int ld_codes, const TtbArState* state, const float* mel_emb,
+                                 const float* mel_pos, int B, int D, int pos_mode, float* x, void* stream) {
+  return ttb_ar_embed_step_rows(codes, ld_codes, state, nullptr, mel_emb, mel_pos, B, D, pos_mode, x, stream);
 }
 
 template <bool TYPICAL>
 static int launch_ar_sample(const char* name, const float* logits, int ld_logits, int V, int B, const float* uniforms,
                             int ld_u, uint32_t* seen, int* codes, int ld_codes, int* finished, TtbArState* state,
                             float temperature, int top_k, float top_p, float rep_penalty, int stop_token, int advance,
-                            float typical_mass, void* stream) {
+                            float typical_mass, const int* row_start, void* stream) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (top_k <= 0 || top_k > 50) { set_error("%s: top_k=%d unsupported (1..50)", name, top_k); return -1; }
   const size_t smem = (size_t)V * sizeof(float);
   if (smem > 40 * 1024) { set_error("%s: vocabulary %d too large", name, V); return -1; }
+  if (row_start && (ld_codes <= 0 || ld_u <= 0)) { set_error("%s: row_start needs ld_codes, ld_u > 0", name); return -1; }
   ar_sample_kernel<TYPICAL><<<B, SAMP_THREADS, smem, st>>>(logits, ld_logits, V, uniforms, ld_u, seen, codes, ld_codes,
                                                            finished, state, temperature, top_k, top_p, rep_penalty,
-                                                           stop_token, advance ? 1 : 0, typical_mass);
+                                                           stop_token, advance ? 1 : 0, typical_mass, row_start);
   TTB_CHECK_LAUNCH("ar_sample_kernel");
   return 0;
 }
@@ -403,7 +416,16 @@ extern "C" int ttb_ar_sample(const float* logits, int ld_logits, int V, int B, c
                              void* stream) {
   return launch_ar_sample<false>("ttb_ar_sample", logits, ld_logits, V, B, uniforms, ld_u, seen, codes, ld_codes,
                                  finished, state, temperature, top_k, top_p, rep_penalty, stop_token, advance, 1.f,
-                                 stream);
+                                 nullptr, stream);
+}
+
+extern "C" int ttb_ar_sample_rows(const float* logits, int ld_logits, int V, int B, const float* uniforms, int ld_u,
+                                  uint32_t* seen, int* codes, int ld_codes, int* finished, TtbArState* state,
+                                  float temperature, int top_k, float top_p, float rep_penalty, int stop_token, int advance,
+                                  const int* row_start, void* stream) {
+  return launch_ar_sample<false>("ttb_ar_sample_rows", logits, ld_logits, V, B, uniforms, ld_u, seen, codes, ld_codes,
+                                 finished, state, temperature, top_k, top_p, rep_penalty, stop_token, advance, 1.f,
+                                 row_start, stream);
 }
 
 extern "C" int ttb_ar_sample_typical(const float* logits, int ld_logits, int V, int B, const float* uniforms, int ld_u,
@@ -416,7 +438,7 @@ extern "C" int ttb_ar_sample_typical(const float* logits, int ld_logits, int V, 
   }
   return launch_ar_sample<true>("ttb_ar_sample_typical", logits, ld_logits, V, B, uniforms, ld_u, seen, codes, ld_codes,
                                 finished, state, temperature, top_k, top_p, rep_penalty, stop_token, advance,
-                                typical_mass, stream);
+                                typical_mass, nullptr, stream);
 }
 
 extern "C" int ttb_ar_fix_codes(int* codes, int B, int L, int stop_token, int* trim_len, void* stream) {

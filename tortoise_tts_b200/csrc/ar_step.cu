@@ -92,7 +92,18 @@ struct AsParams {
   unsigned long long* bar;                // [0] barrier epoch at launch; arrival slots at [16 * (1 + k)], k < 16
   unsigned int* tickets;                  // [AS_MAX_TILES]
   int attn_data_bytes;                    // compact attention launch: rings of the active warps + the prompt of one head
+  const int* row_start;                   // device [B] or NULL (TtbArStepArgs.row_start)
 };
+
+// Row b's own step: state->step without row_start, else step - row_start[b] clamped to [1, Nmax] (include/ttb.h), so
+// that an idle row of a stream pool never indexes outside its codes and KV rows. ROWS = false compiles the row_start
+// checks away: the launches without row_start (ar_step_kernel<false>, ar_attn_only_kernel<false>,
+// ar_attn_compact_kernel<false>) are the kernels they were before row_start existed (a runtime branch in ar_step_kernel
+// cost its one-row decode 1-2 % on H100).
+template <bool ROWS>
+TTB_DEVINL int row_step(const AsParams& p, int step, int b) {
+  return (ROWS && p.row_start) ? min(max(step - __ldg(p.row_start + b), 1), p.Nmax) : step;
+}
 
 // phase bits (phase_mask)
 enum { PH_EMBED = 1, PH_QKV = 2, PH_ATTN = 4, PH_PROJ = 8, PH_LN2 = 16, PH_FC = 32, PH_PROJ2 = 64, PH_LN1 = 128, PH_HEAD = 256,
@@ -497,15 +508,15 @@ TTB_DEVINL void mma_chunk(MmaState& st, const uint32_t* qb, uint32_t kt, uint32_
 // `wait_pdl`: the caller has NOT yet executed griddepcontrol.wait (ar_attn_only_kernel under programmatic dependent
 // launch): the prompt prefix and the first candidate tiles are requested first -- the caches were written by earlier
 // steps / this step's earlier kernels, only q and the new K / V come from the c_attn GEMM this launch depends on.
-template <class CtrlT>
+template <bool ROWS, class CtrlT>
 TTB_DEVINL void attn_phase_mma(const AsParams& p, int layer, uint8_t* data, CtrlT* ctrl, AsRole& rl, bool wait_pdl = false) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   int* err = &p.state->reserved[0];
   const int B = p.B, H = p.H, Nmax = p.Nmax, D = p.H * 64;
   constexpr int NS = AS_RING_NS;
   constexpr int CHUNK_BYTES = AS_CHUNK_BYTES;          // K tile 2 KB | V tile 2 KB
-  const int slot = p.state->step - 1;
-  const int nold = slot;
+  const int step = p.state->step;
+  const int slot0 = step - 1;                          // KV slot and candidate length of every row without row_start
   uint8_t* ring = data + warp * NS * CHUNK_BYTES;
   uint8_t* prefix_s = data + p.ipr * p.team * NS * CHUNK_BYTES;   // behind the rings of the active warps (host checks the fit)
   const CUtensorMap* map_c = p.maps + 4 * p.L + 5;
@@ -514,9 +525,10 @@ TTB_DEVINL void attn_phase_mma(const AsParams& p, int layer, uint8_t* data, Ctrl
   for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
     // the unit's group: the last g with u0 <= u, by bisection over [g, ngroups) (a CTA's units only grow, so its group
     // only advances). One group (every tts() call): the values come from the parameters; reading the table here cost
-    // ~2 % of the one-row decode of 603 tokens on H100
+    // ~2 % of the one-row decode of 603 tokens on H100. With row_start the table is read even for one group: a stream
+    // pool rewrites its groups' P between steps (ttb_ar_step_set_group_len)
     int gb0 = 0, gB = B, ncph = p.ncph0, P = p.P0, lu = u;
-    if (p.ngroups > 1) {
+    if (p.ngroups > 1 || (ROWS && p.row_start)) {
       for (int hi = p.ngroups; hi - g > 1;) {
         const int mid = (g + hi) >> 1;
         if (__ldg(&p.gtab[mid].u0) <= u) g = mid; else hi = mid;
@@ -539,11 +551,12 @@ TTB_DEVINL void attn_phase_mma(const AsParams& p, int layer, uint8_t* data, Ctrl
       }
     }
     const int sub = warp % p.team;
-    const int nch = (nold + 15) / 16;
+    const int nch0 = (slot0 + 15) / 16;
     // first NS tiles of candidate bb's stream into this warp's ring (lane 0). All stages are free whenever this is
     // called: at the start of the unit, or after the last tile of the previous item was consumed.
     auto issue_head = [&](int bb) {
       const int it = (layer * B + bb) * H + h;
+      const int nch = ROWS ? (row_step<ROWS>(p, step, bb) - 1 + 15) / 16 : nch0;   // chunks of bb's own length
       for (int s = 0; s < NS; ++s) {
         const int c = sub + s * p.team;
         if (c < nch) {
@@ -567,6 +580,9 @@ TTB_DEVINL void attn_phase_mma(const AsParams& p, int layer, uint8_t* data, Ctrl
       if (valid && !head_issued && lane == 0) issue_head(b);
       if (wait_pdl) { pdl_wait(); wait_pdl = false; }
       if (valid) {
+        const int slot = ROWS ? row_step<ROWS>(p, step, b) - 1 : slot0;   // KV slot written = positions before it
+        const int nold = slot;
+        const int nch = ROWS ? (nold + 15) / 16 : nch0;
         const __nv_bfloat16* qrow = p.qkv + (long long)b * 3 * D + h * 64;
         // q as the B operand of the score MMA: column 0 <-> lanes 0-3; b0 = dims 16 ks + 2 lane (+1), b1 = + 8
         uint32_t qb[8];
@@ -681,6 +697,7 @@ TTB_DEVINL void attn_phase_mma(const AsParams& p, int layer, uint8_t* data, Ctrl
 // mode 0: x = mel_emb[tok] + mel_pos[pos]        (ar_embed_step)
 // mode 1: x += rbias + sum_s part[s]             (residual update folded with the split-K reduction)
 // then y = LN(x; g1, b1) [-> LN(.; g2, b2)] -> bf16 out
+template <bool ROWS>
 TTB_DEVINL void ln_phase(const AsParams& p, int mode, const float* part, int nsplit, int ldp, const float* __restrict__ rbias,
                          const float* __restrict__ g1, const float* __restrict__ b1, const float* __restrict__ g2,
                          const float* __restrict__ b2, __nv_bfloat16* out, AsCtrl* ctrl) {
@@ -690,7 +707,7 @@ TTB_DEVINL void ln_phase(const AsParams& p, int mode, const float* part, int nsp
   for (int row = blockIdx.x; row < p.B; row += gridDim.x) {
     float v[2];
     if (mode == 0) {
-      const int j = p.state->step;
+      const int j = row_step<ROWS>(p, p.state->step, row);
       const int tok = p.codes[(long long)row * p.ld_codes + j - 1];
       const int pos = p.pos_mode ? j + 1 : j;          // autoregressive.py:147-149 (SURVEY App. D-1)
 #pragma unroll
@@ -755,6 +772,7 @@ TTB_DEVINL void ln_phase(const AsParams& p, int mode, const float* part, int nsp
 }
 
 // ------------------------------------------------------------------ the step kernel
+template <bool ROWS>
 __global__ void __launch_bounds__(AS_THREADS, 1) ar_step_kernel(const __grid_constant__ AsParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* data = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -791,7 +809,7 @@ __global__ void __launch_bounds__(AS_THREADS, 1) ar_step_kernel(const __grid_con
   if (p.phase_mask & PH_EMBED) {
     if (pf && L0 < L1) prefetch_gemm_item(p, p.maps + 4 * L0 + G_QKV, p.g[G_QKV]);
     const AsLayer& l0 = p.layers[L0 < p.L ? L0 : 0];
-    ln_phase(p, 0, nullptr, 0, 0, nullptr, l0.ln1_g, l0.ln1_b, nullptr, nullptr, p.a, ctrl);
+    ln_phase<ROWS>(p, 0, nullptr, 0, 0, nullptr, l0.ln1_g, l0.ln1_b, nullptr, nullptr, p.a, ctrl);
     grid_sync(p, rl);
   }
   for (int l = L0; l < L1; ++l) {
@@ -803,7 +821,7 @@ __global__ void __launch_bounds__(AS_THREADS, 1) ar_step_kernel(const __grid_con
       AS_SYNC_UNLESS_LAST(1, l);
     }
     if (p.phase_mask & PH_ATTN) {
-      attn_phase_mma(p, l, data, ctrl, rl);
+      attn_phase_mma<ROWS>(p, l, data, ctrl, rl);
       AS_SYNC_UNLESS_LAST(2, l);
     }
     if (p.phase_mask & PH_NOP) grid_sync(p, rl);
@@ -813,7 +831,7 @@ __global__ void __launch_bounds__(AS_THREADS, 1) ar_step_kernel(const __grid_con
       AS_SYNC_UNLESS_LAST(3, l);
     }
     if (p.phase_mask & PH_LN2) {
-      ln_phase(p, 1, p.part, p.g[G_PROJ].nsplit, p.g[G_PROJ].ldp, lw.bproj, lw.ln2_g, lw.ln2_b, nullptr, nullptr, p.a, ctrl);
+      ln_phase<ROWS>(p, 1, p.part, p.g[G_PROJ].nsplit, p.g[G_PROJ].ldp, lw.bproj, lw.ln2_g, lw.ln2_b, nullptr, nullptr, p.a, ctrl);
       AS_SYNC_UNLESS_LAST(4, l);
     }
     if (p.phase_mask & PH_FC) {
@@ -831,9 +849,9 @@ __global__ void __launch_bounds__(AS_THREADS, 1) ar_step_kernel(const __grid_con
     if (p.phase_mask & PH_LN1) {
       if (l + 1 < p.L) {
         const AsLayer& nx = p.layers[l + 1];
-        ln_phase(p, 1, p.part, p.g[G_PROJ2].nsplit, p.g[G_PROJ2].ldp, lw.bproj2, nx.ln1_g, nx.ln1_b, nullptr, nullptr, p.a, ctrl);
+        ln_phase<ROWS>(p, 1, p.part, p.g[G_PROJ2].nsplit, p.g[G_PROJ2].ldp, lw.bproj2, nx.ln1_g, nx.ln1_b, nullptr, nullptr, p.a, ctrl);
       } else {
-        ln_phase(p, 1, p.part, p.g[G_PROJ2].nsplit, p.g[G_PROJ2].ldp, lw.bproj2, p.lnf_g, p.lnf_b, p.fn_g, p.fn_b, p.hn, ctrl);
+        ln_phase<ROWS>(p, 1, p.part, p.g[G_PROJ2].nsplit, p.g[G_PROJ2].ldp, lw.bproj2, p.lnf_g, p.lnf_b, p.fn_g, p.fn_b, p.hn, ctrl);
       }
       AS_SYNC_UNLESS_LAST(7, l);
     }
@@ -849,6 +867,7 @@ __global__ void __launch_bounds__(AS_THREADS, 1) ar_step_kernel(const __grid_con
 
 // The attention phase alone as an ordinary (non-cooperative) launch: no grid barrier. Used by the "mixed" decode
 // mode, where the GEMMs / LayerNorms of the step stay separate kernels (see ar_engine.py).
+template <bool ROWS>
 __global__ void __launch_bounds__(AS_THREADS, 1) ar_attn_only_kernel(const __grid_constant__ AsParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* data = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -863,7 +882,7 @@ __global__ void __launch_bounds__(AS_THREADS, 1) ar_attn_only_kernel(const __gri
   AsRole rl;
   rl.stage = 0; rl.phase = 0; rl.prefix_par = 0; rl.bar_target = 0;
   rl.ring_par[0] = rl.ring_par[1] = 0;
-  attn_phase_mma(p, p.layer_begin, data, ctrl, rl, true);   // waits for the c_attn GEMM (PDL) after its first requests
+  attn_phase_mma<ROWS>(p, p.layer_begin, data, ctrl, rl, true);   // waits for the c_attn GEMM (PDL) after its first requests
   pdl_launch_dependents();
 }
 
@@ -873,6 +892,7 @@ __global__ void __launch_bounds__(AS_THREADS, 1) ar_attn_only_kernel(const __gri
 // (prompts up to 176 positions), which gives the SM its 16 concurrent KV streams back when the kernel has it to itself. Used when the candidates are decoded
 // as two independent half-batches on two streams (ar_engine.py, TTB_AR_CHAINS): the latency-bound GEMM / LayerNorm
 // chain of one half then overlaps the bandwidth-bound attention of the other.
+template <bool ROWS>
 __global__ void __launch_bounds__(AS_COMPACT_WARPS * 32, AS_COMPACT_CTAS) ar_attn_compact_kernel(const __grid_constant__ AsParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* data = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -887,21 +907,26 @@ __global__ void __launch_bounds__(AS_COMPACT_WARPS * 32, AS_COMPACT_CTAS) ar_att
   AsRole rl;
   rl.stage = 0; rl.phase = 0; rl.prefix_par = 0; rl.bar_target = 0;
   rl.ring_par[0] = rl.ring_par[1] = 0;
-  attn_phase_mma(p, p.layer_begin, data, ctrl, rl, true);
+  attn_phase_mma<ROWS>(p, p.layer_begin, data, ctrl, rl, true);
   pdl_launch_dependents();
 }
 
-// prompt K/V from a qkv buffer [P, 3*H*64] into the interleaved prefix cache [H][P][K 64 | V 64]
-__global__ void ar_step_store_prefix_kernel(const __nv_bfloat16* __restrict__ qkv, int P, int H, __nv_bfloat16* __restrict__ pkv) {
+// prompt K/V from a qkv buffer [P, 3*H*64] into the interleaved prefix cache [H][cap][K 64 | V 64] (cap >= P positions
+// per head: a stream pool's slot buffers are sized for the longest prompt)
+__global__ void ar_step_store_prefix_kernel(const __nv_bfloat16* __restrict__ qkv, int P, int cap, int H,
+                                            __nv_bfloat16* __restrict__ pkv) {
   const int D = H * 64;
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;  // over P * D
   if (i >= (long long)P * D) return;
   const int pp = (int)(i / D), c = (int)(i - (long long)pp * D);
   const int h = c >> 6, d = c & 63;
-  __nv_bfloat16* dst = pkv + ((long long)h * P + pp) * 128;
+  __nv_bfloat16* dst = pkv + ((long long)h * cap + pp) * 128;
   dst[d] = qkv[(long long)pp * 3 * D + D + c];
   dst[64 + d] = qkv[(long long)pp * 3 * D + 2 * D + c];
 }
+
+// one group's prompt length in the device group table (ttb_ar_step_set_group_len); stream-ordered, graph-free
+__global__ void ar_step_set_group_len_kernel(AsGroup* gtab, int g, int P) { gtab[g].P = P; }
 
 // ------------------------------------------------------------------ host: plan
 struct AsPlan {
@@ -1110,9 +1135,12 @@ extern "C" int ttb_ar_step_setup(const TtbArStepArgs* ap, void* stream) {
   if (e != cudaSuccess) return check_cuda(e, "ttb_ar_step_setup");
   static bool attr_set = false;
   if (!attr_set) {
-    e = cudaFuncSetAttribute(ar_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AS_SMEM_TOTAL);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(ar_attn_only_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AS_SMEM_TOTAL);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(ar_attn_compact_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AS_SMEM_TOTAL);
+    e = cudaFuncSetAttribute(ar_step_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, AS_SMEM_TOTAL);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(ar_step_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, AS_SMEM_TOTAL);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(ar_attn_only_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, AS_SMEM_TOTAL);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(ar_attn_only_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, AS_SMEM_TOTAL);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(ar_attn_compact_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, AS_SMEM_TOTAL);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(ar_attn_compact_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, AS_SMEM_TOTAL);
     if (e != cudaSuccess) return check_cuda(e, "cudaFuncSetAttribute(ar_step_kernel)");
     attr_set = true;
   }
@@ -1138,20 +1166,24 @@ extern "C" int ttb_ar_decode_step(const TtbArStepArgs* ap, void* stream) {
   p.part = a.part; p.logits = a.logits;
   p.prefix_kv = reinterpret_cast<const __nv_bfloat16*>(a.prefix_kv);
   p.cand_kv = reinterpret_cast<__nv_bfloat16*>(a.cand_kv);
+  p.row_start = a.row_start;
   p.bar = reinterpret_cast<unsigned long long*>(a.sync);
   p.tickets = reinterpret_cast<unsigned int*>(reinterpret_cast<unsigned char*>(a.sync) + AS_SYNC_BAR_BYTES);
   if (p.phase_mask == PH_ATTN && p.layer_end == p.layer_begin + 1) {
     const int units = p.units;
     if (a.attn_compact) {
       const int cgrid = pl.grid * AS_COMPACT_CTAS;
-      const cudaError_t lc = launch_pdl(ar_attn_compact_kernel, dim3(units < cgrid ? units : cgrid), dim3(AS_COMPACT_WARPS * 32),
-                                        (size_t)(p.attn_data_bytes + AS_CTRL_COMPACT_BYTES + 1024), st, p);
+      const dim3 grid(units < cgrid ? units : cgrid), block(AS_COMPACT_WARPS * 32);
+      const size_t smem = (size_t)(p.attn_data_bytes + AS_CTRL_COMPACT_BYTES + 1024);
+      const cudaError_t lc = a.row_start ? launch_pdl(ar_attn_compact_kernel<true>, grid, block, smem, st, p)
+                                         : launch_pdl(ar_attn_compact_kernel<false>, grid, block, smem, st, p);
       if (lc != cudaSuccess) return check_cuda(lc, "ar_attn_compact_kernel launch");
       TTB_CHECK_LAUNCH("ar_attn_compact_kernel");
       return 0;
     }
-    const cudaError_t la = launch_pdl(ar_attn_only_kernel, dim3(units < pl.grid ? units : pl.grid), dim3(AS_THREADS),
-                                      (size_t)AS_SMEM_TOTAL, st, p);
+    const dim3 grid(units < pl.grid ? units : pl.grid), block(AS_THREADS);
+    const cudaError_t la = a.row_start ? launch_pdl(ar_attn_only_kernel<true>, grid, block, (size_t)AS_SMEM_TOTAL, st, p)
+                                       : launch_pdl(ar_attn_only_kernel<false>, grid, block, (size_t)AS_SMEM_TOTAL, st, p);
     if (la != cudaSuccess) return check_cuda(la, "ar_attn_only_kernel launch");
     TTB_CHECK_LAUNCH("ar_attn_only_kernel");
     return 0;
@@ -1166,17 +1198,41 @@ extern "C" int ttb_ar_decode_step(const TtbArStepArgs* ap, void* stream) {
   at[0].val.cooperative = 1;
   cfg.attrs = at;
   cfg.numAttrs = 1;
-  const cudaError_t le = cudaLaunchKernelEx(&cfg, ar_step_kernel, p);
+  const cudaError_t le = a.row_start ? cudaLaunchKernelEx(&cfg, ar_step_kernel<true>, p)
+                                     : cudaLaunchKernelEx(&cfg, ar_step_kernel<false>, p);
   if (le != cudaSuccess) return check_cuda(le, "ar_step_kernel launch");
   TTB_CHECK_LAUNCH("ar_step_kernel");
   return 0;
 }
 
-extern "C" int ttb_ar_step_store_prefix(const void* qkv, int P, int H, void* prefix_kv, void* stream) {
+extern "C" int ttb_ar_step_store_prefix_cap(const void* qkv, int P, int cap, int H, void* prefix_kv, void* stream) {
+  if (P <= 0 || cap < P) { set_error("ttb_ar_step_store_prefix_cap: P=%d, cap=%d (need 0 < P <= cap)", P, cap); return -1; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long long n = (long long)P * H * 64;
-  ar_step_store_prefix_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(qkv), P, H,
-                                                                          reinterpret_cast<__nv_bfloat16*>(prefix_kv));
+  ar_step_store_prefix_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(qkv), P, cap,
+                                                                          H, reinterpret_cast<__nv_bfloat16*>(prefix_kv));
   TTB_CHECK_LAUNCH("ar_step_store_prefix_kernel");
+  return 0;
+}
+
+extern "C" int ttb_ar_step_store_prefix(const void* qkv, int P, int H, void* prefix_kv, void* stream) {
+  return ttb_ar_step_store_prefix_cap(qkv, P, P, H, prefix_kv, stream);
+}
+
+extern "C" int ttb_ar_step_set_group_len(const TtbArStepArgs* ap, int group, int P, void* stream) {
+  const TtbArStepArgs& a = *ap;
+  AsPlan pl;
+  if (make_plan(a, pl)) return -1;
+  if (!a.tables || group < 0 || group >= pl.ngroups) {
+    set_error("ttb_ar_step_set_group_len: group %d of %d (or no tables)", group, pl.ngroups);
+    return -1;
+  }
+  if (P <= 0 || P > pl.gtab[group].P) {
+    set_error("ttb_ar_step_set_group_len: P=%d outside (0, %d], the prefix capacity of group %d", P, pl.gtab[group].P, group);
+    return -1;
+  }
+  AsGroup* gtab = reinterpret_cast<AsGroup*>(reinterpret_cast<unsigned char*>(a.tables) + group_table_offset(a.L, pl.ngroups));
+  ar_step_set_group_len_kernel<<<1, 1, 0, static_cast<cudaStream_t>(stream)>>>(gtab, group, P);
+  TTB_CHECK_LAUNCH("ar_step_set_group_len_kernel");
   return 0;
 }

@@ -163,11 +163,13 @@ template <int NV>
 __global__ void __launch_bounds__(64)
 ar_capture_latents_kernel(const float* __restrict__ x, int B, int D, const float* __restrict__ g1,
                           const float* __restrict__ b1, const float* __restrict__ g2, const float* __restrict__ b2,
-                          const TtbArState* __restrict__ state, int Nmax, float* __restrict__ out, long long ld_row) {
+                          const TtbArState* __restrict__ state, int Nmax, float* __restrict__ out, long long ld_row,
+                          const int* __restrict__ row_start) {
   const int lane = threadIdx.x & 31;
   const long long row = (long long)blockIdx.x * 2 + (threadIdx.x >> 5);
-  const int j = state->step - 1;
-  if (row >= B || j < 0 || j >= Nmax) return;
+  if (row >= B) return;
+  const int j = state->step - 1 - (row_start ? row_start[row] : 0);
+  if (j < 0 || j >= Nmax) return;
   const float* xr = x + row * D;
   float4 v[NV];
 #pragma unroll
@@ -553,22 +555,22 @@ extern "C" int ttb_residual_layernorm(float* x, int M, int D, const float* parti
   return 0;
 }
 
-extern "C" int ttb_ar_capture_latents(const float* x, int B, int D, const float* g1, const float* b1, const float* g2,
-                                      const float* b2, const TtbArState* state, int Nmax, float* out, long long ld_row,
-                                      void* stream) {
+extern "C" int ttb_ar_capture_latents_rows(const float* x, int B, int D, const float* g1, const float* b1,
+                                           const float* g2, const float* b2, const TtbArState* state, int Nmax, float* out,
+                                           long long ld_row, const int* row_start, void* stream) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (B <= 0) return 0;
   const void* ptrs[] = {x, g1, b1, g2, b2, out};
   bool aligned = (ld_row & 3) == 0 && ld_row >= (long long)Nmax * D;
   for (const void* p : ptrs) aligned = aligned && p && !(reinterpret_cast<uintptr_t>(p) & 15);
   if (D % 128 != 0 || D > 1024 || Nmax <= 0 || !state || !aligned) {
-    set_error("ttb_ar_capture_latents: needs D a multiple of 128 <= 1024 (D=%d), Nmax > 0, ld_row >= Nmax * D, a multiple "
+    set_error("ttb_ar_capture_latents_rows: needs D a multiple of 128 <= 1024 (D=%d), Nmax > 0, ld_row >= Nmax * D, a multiple "
               "of 4, and 16-byte aligned pointers", D);
     return -1;
   }
   const dim3 grid((B + 1) / 2);
 #define TTB_CAP_CASE(NV)                                                                                             \
-  case NV: ar_capture_latents_kernel<NV><<<grid, 64, 0, st>>>(x, B, D, g1, b1, g2, b2, state, Nmax, out, ld_row); break;
+  case NV: ar_capture_latents_kernel<NV><<<grid, 64, 0, st>>>(x, B, D, g1, b1, g2, b2, state, Nmax, out, ld_row, row_start); break;
   switch (D / 128) {
     TTB_CAP_CASE(1) TTB_CAP_CASE(2) TTB_CAP_CASE(3) TTB_CAP_CASE(4) TTB_CAP_CASE(5) TTB_CAP_CASE(6) TTB_CAP_CASE(7)
     TTB_CAP_CASE(8)
@@ -576,6 +578,12 @@ extern "C" int ttb_ar_capture_latents(const float* x, int B, int D, const float*
 #undef TTB_CAP_CASE
   TTB_CHECK_LAUNCH("ar_capture_latents_kernel");
   return 0;
+}
+
+extern "C" int ttb_ar_capture_latents(const float* x, int B, int D, const float* g1, const float* b1, const float* g2,
+                                      const float* b2, const TtbArState* state, int Nmax, float* out, long long ld_row,
+                                      void* stream) {
+  return ttb_ar_capture_latents_rows(x, B, D, g1, b1, g2, b2, state, Nmax, out, ld_row, nullptr, stream);
 }
 
 extern "C" int ttb_rmsnorm(const float* x, int M, int D, const float* g, void* out_bf16, void* stream) {

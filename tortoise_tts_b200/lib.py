@@ -64,7 +64,7 @@ class ArStepArgs(C.Structure):
                 ("debug_layer_begin", C.c_int), ("debug_layer_end", C.c_int), ("debug_phase_mask", C.c_int),
                 ("attn_compact", C.c_int),
                 ("groups", C.c_int), ("group_begin", C.POINTER(C.c_int)), ("group_P", C.POINTER(C.c_int)),
-                ("group_prefix_kv", C.POINTER(C.c_void_p))]
+                ("group_prefix_kv", C.POINTER(C.c_void_p)), ("row_start", C.c_void_p)]
 
 
 _lib = None
@@ -81,6 +81,8 @@ SYMBOLS = [
     "ttb_audio_resample", "ttb_audio_stft_mel", "ttb_mean_rows", "ttb_equal_linear",
     "ttb_pair_exchange", "ttb_enable_peer_access", "ttb_peer_alloc", "ttb_peer_open", "ttb_peer_close", "ttb_peer_free",
     "ttb_wav2vec_conv0", "ttb_layernorm_act", "ttb_argmax_rows", "ttb_ar_sample_typical", "ttb_ar_capture_latents",
+    "ttb_ar_embed_step_rows", "ttb_ar_sample_rows", "ttb_ar_capture_latents_rows", "ttb_ar_step_store_prefix_cap",
+    "ttb_ar_step_set_group_len",
 ]
 
 
@@ -210,9 +212,14 @@ def attention(qkv, out, *, nseq, T, H, ld, ldo, k_off, v_off, scale, causal=Fals
     _chk(load().ttb_attention(C.byref(a), _stream()), "ttb_attention")
 
 
-def ar_embed_step(codes, ld_codes, state, mel_emb, mel_pos, B, D, pos_mode, x):
-    _chk(load().ttb_ar_embed_step(_p(codes), ld_codes, _p(state), _p(mel_emb), _p(mel_pos), B, D, pos_mode, _p(x),
-                                  _stream()), "ttb_ar_embed_step")
+def ar_embed_step(codes, ld_codes, state, mel_emb, mel_pos, B, D, pos_mode, x, row_start=None):
+    """`row_start` (int32 [B] or None): per-row start steps (include/ttb.h ttb_ar_embed_step_rows)."""
+    if row_start is None:
+        _chk(load().ttb_ar_embed_step(_p(codes), ld_codes, _p(state), _p(mel_emb), _p(mel_pos), B, D, pos_mode, _p(x),
+                                      _stream()), "ttb_ar_embed_step")
+        return
+    _chk(load().ttb_ar_embed_step_rows(_p(codes), ld_codes, _p(state), _p(row_start), _p(mel_emb), _p(mel_pos), B, D,
+                                       pos_mode, _p(x), _stream()), "ttb_ar_embed_step_rows")
 
 
 def ar_decode_attention(qkv, pk, pv, ck, cv, state, B, H, P, Nmax, out, scratch_o, scratch_lse):
@@ -225,8 +232,13 @@ def ar_store_prefix(qkv, P, H, pk, pv):
     _chk(load().ttb_ar_store_prefix(_p(_bf(qkv)), P, H, _p(_bf(pk)), _p(_bf(pv)), _stream()), "ttb_ar_store_prefix")
 
 
-def ar_step_store_prefix(qkv, P, H, pkv):
-    _chk(load().ttb_ar_step_store_prefix(_p(_bf(qkv)), P, H, _p(_bf(pkv)), _stream()), "ttb_ar_step_store_prefix")
+def ar_step_store_prefix(qkv, P, H, pkv, cap=None):
+    """`cap`: positions per head of `pkv` when it is larger than P (a stream pool's slot prefix)."""
+    if cap is None:
+        _chk(load().ttb_ar_step_store_prefix(_p(_bf(qkv)), P, H, _p(_bf(pkv)), _stream()), "ttb_ar_step_store_prefix")
+        return
+    _chk(load().ttb_ar_step_store_prefix_cap(_p(_bf(qkv)), P, cap, H, _p(_bf(pkv)), _stream()),
+         "ttb_ar_step_store_prefix_cap")
 
 
 AR_STEP_MAX_B, AR_STEP_MAX_P, AR_STEP_MAX_D = 256, 352, 1024    # limits of csrc/ar_step.cu (make_plan)
@@ -241,14 +253,15 @@ class ArStep:
     """Handle of the one-kernel decode step (include/ttb.h TtbArStepArgs): owns the scratch / table / sync buffers and
     keeps every tensor the kernel points at alive. `layers`: list of dicts with the keys of ARWeights.layers.
     `groups`: None (every row attends to `prefix_kv` of P positions) or a list of (row_begin, row_end, P_g, prefix_kv_g)
-    covering rows [0, B) in order; `P` and `prefix_kv` are then ignored."""
+    covering rows [0, B) in order; `P` and `prefix_kv` are then ignored. `row_start`: None or a device int32 [B] of
+    per-row start steps (include/ttb.h TtbArStepArgs.row_start)."""
 
     def __init__(self, *, B, D, H, L, V, P, Nmax, pos_mode, layers, w_head, b_head, lnf_g, lnf_b, fn_g, fn_b, mel_emb,
                  mel_pos, codes, ld_codes, state, x, a, qkv, o, h, hn, logits, prefix_kv, cand_kv, attn_compact=False,
-                 groups=None):
+                 groups=None, row_start=None):
         dev = x.device
         self._keep = (layers, w_head, b_head, lnf_g, lnf_b, fn_g, fn_b, mel_emb, mel_pos, codes, state, x, a, qkv, o, h,
-                      hn, logits, prefix_kv, cand_kv, groups)
+                      hn, logits, prefix_kv, cand_kv, groups, row_start)
         self._larr = (ArStepLayer * L)()
         for i, lw in enumerate(layers):
             for n in ("wqkv", "wproj", "wfc", "wproj2"):
@@ -266,6 +279,9 @@ class ArStep:
         g.h, g.hn, g.logits = _bf(h).data_ptr(), _bf(hn).data_ptr(), _f32(logits).data_ptr()
         g.prefix_kv, g.cand_kv = _bf(prefix_kv).data_ptr(), _bf(cand_kv).data_ptr()
         g.attn_compact = 1 if attn_compact else 0
+        if row_start is not None:
+            assert row_start.dtype == torch.int32 and row_start.numel() == B, (row_start.dtype, row_start.shape)
+            g.row_start = row_start.data_ptr()
         if groups:
             n = len(groups)
             self._gbeg = (C.c_int * (n + 1))(*([int(r[0]) for r in groups] + [int(groups[-1][1])]))
@@ -290,12 +306,21 @@ class ArStep:
         g.debug_phase_mask, g.debug_layer_begin, g.debug_layer_end = phase_mask, layer_begin, layer_end
         _chk(load().ttb_ar_decode_step(C.byref(g), _stream()), "ttb_ar_decode_step")
 
+    def set_group_len(self, group, P):
+        """Prompt length of one group, written into the device group table on the current stream (no new setup or
+        graph capture); P at most the group's P at construction (its prefix capacity)."""
+        _chk(load().ttb_ar_step_set_group_len(C.byref(self.args), int(group), int(P), _stream()), "ttb_ar_step_set_group_len")
+
 
 def ar_sample(logits, ld_logits, V, B, uniforms, ld_u, seen, codes, ld_codes, finished, state, temperature, top_k,
-              top_p, rep_penalty, stop_token, advance=True):
-    _chk(load().ttb_ar_sample(_p(_f32(logits)), ld_logits, V, B, _p(_f32(uniforms)), ld_u, _p(seen), _p(codes), ld_codes,
-                              _p(finished), _p(state), C.c_float(temperature), top_k, C.c_float(top_p),
-                              C.c_float(rep_penalty), stop_token, 1 if advance else 0, _stream()), "ttb_ar_sample")
+              top_p, rep_penalty, stop_token, advance=True, row_start=None):
+    args = (_p(_f32(logits)), ld_logits, V, B, _p(_f32(uniforms)), ld_u, _p(seen), _p(codes), ld_codes, _p(finished),
+            _p(state), C.c_float(temperature), top_k, C.c_float(top_p), C.c_float(rep_penalty), stop_token,
+            1 if advance else 0)
+    if row_start is None:
+        _chk(load().ttb_ar_sample(*args, _stream()), "ttb_ar_sample")
+    else:
+        _chk(load().ttb_ar_sample_rows(*args, _p(row_start), _stream()), "ttb_ar_sample_rows")
 
 
 def ar_sample_typical(logits, ld_logits, V, B, uniforms, ld_u, seen, codes, ld_codes, finished, state, temperature,
@@ -307,11 +332,16 @@ def ar_sample_typical(logits, ld_logits, V, B, uniforms, ld_u, seen, codes, ld_c
                                       _stream()), "ttb_ar_sample_typical")
 
 
-def ar_capture_latents(x, B, D, g1, b1, g2, b2, state, Nmax, out, ld_row):
+def ar_capture_latents(x, B, D, g1, b1, g2, b2, state, Nmax, out, ld_row, row_start=None):
     """out[b, state.step - 1] = final_norm(ln_f(x[b])) for the B rows of a decode step, enqueued after its sampler
-    (include/ttb.h ttb_ar_capture_latents); `ld_row` = fp32 elements between the rows of `out`."""
-    _chk(load().ttb_ar_capture_latents(_p(_f32(x)), B, D, _p(_f32(g1)), _p(_f32(b1)), _p(_f32(g2)), _p(_f32(b2)), _p(state),
-                                       Nmax, _p(_f32(out)), C.c_longlong(ld_row), _stream()), "ttb_ar_capture_latents")
+    (include/ttb.h ttb_ar_capture_latents); `ld_row` = fp32 elements between the rows of `out`. `row_start`: per-row
+    start steps (column state.step - 1 - row_start[b])."""
+    args = (_p(_f32(x)), B, D, _p(_f32(g1)), _p(_f32(b1)), _p(_f32(g2)), _p(_f32(b2)), _p(state), Nmax, _p(_f32(out)),
+            C.c_longlong(ld_row))
+    if row_start is None:
+        _chk(load().ttb_ar_capture_latents(*args, _stream()), "ttb_ar_capture_latents")
+    else:
+        _chk(load().ttb_ar_capture_latents_rows(*args, _p(row_start), _stream()), "ttb_ar_capture_latents_rows")
 
 
 def ar_fix_codes(codes, B, L, stop_token, trim_len):
