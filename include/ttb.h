@@ -191,6 +191,22 @@ int ttb_ar_sample_typical(const float* logits, int ld_logits, int V, int B, cons
                           uint32_t* seen, int* codes, int ld_codes, int* finished, TtbArState* state, float temperature,
                           int top_k, float top_p, float rep_penalty, int stop_token, int advance, float typical_mass,
                           void* stream);
+/* Sampling settings of one row (32 bytes), for ttb_ar_sample_params. temperature > 0, top_k in 1..50, top_p in (0, 1],
+ * rep_penalty > 0, as for ttb_ar_sample. typical_mass == 0 turns the typical-set filter off for that row; in (0, 1] it
+ * is the mass of ttb_ar_sample_typical. reserved: set to 0. */
+typedef struct TtbSampleParams {
+  float temperature, top_p, rep_penalty, typical_mass;
+  int top_k;
+  int reserved[3];
+} TtbSampleParams;
+/* ttb_ar_sample with settings per row: row b reads params[b], a device array [B] (not kernel parameters, so a captured
+ * graph keeps its launch while the table changes). Row b computes what ttb_ar_sample (typical_mass == 0) or
+ * ttb_ar_sample_typical gives with those settings, bit for bit. row_start as for ttb_ar_sample_rows (NULL: every row at
+ * state->step; else ld_codes, ld_u > 0), also with the typical filter. The kernel clamps top_k to [1, 50]; the other
+ * values are not checked on the device: the caller validates the table. */
+int ttb_ar_sample_params(const float* logits, int ld_logits, int V, int B, const float* uniforms, int ld_u,
+                         uint32_t* seen, int* codes, int ld_codes, int* finished, TtbArState* state,
+                         const TtbSampleParams* params, int stop_token, int advance, const int* row_start, void* stream);
 /* The latent the reference's streaming generator yields next to each token (stream_generator.py:982,
  * final_norm(hidden_states[-1][:, -1]) of the step that sampled it), taken from the decode step itself: for every row b,
  * out[b * ld_row + j * D + c] = final_norm(ln_f(x[b, :]))[c] with j = state->step - 1. x fp32 [B, D] is the residual

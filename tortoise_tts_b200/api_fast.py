@@ -58,6 +58,34 @@ def stream_flushes(n, flushed, ended, stream_chunk_size):
     return ([False] if due else []) + ([True] if ended else [])
 
 
+STREAM_SETTINGS = ("temperature", "top_p", "top_k", "repetition_penalty", "length_penalty")   # per stream / per text
+BATCH_SETTINGS = STREAM_SETTINGS + ("typical_sampling", "typical_mass")                      # per sentence of tts_batch
+
+
+def row_settings(kwargs_list, n, base, allowed):
+    """The per-text sampling settings of a batch: `kwargs_list` (one dict per text, keys from `allowed`) over `base` (the
+    call's own settings, a dict with every key of `allowed`), validated before any work starts: a list whose length is
+    not n raises ValueError, a key outside `allowed` TypeError, a bad value ValueError (lib.sample_params_row). Returns
+    one dict per text for the engine (temperature, top_k, top_p, repetition_penalty, typical_mass);
+    length_penalty is accepted and has no effect, as in tts_stream."""
+    kwargs_list = list(kwargs_list)
+    if len(kwargs_list) != n:
+        raise ValueError("kwargs_list has %d entries for %d texts" % (len(kwargs_list), n))
+    out = []
+    for u, kw in enumerate(kwargs_list):
+        unknown = set(kw) - set(allowed)
+        if unknown:
+            raise TypeError("kwargs_list[%d]: unsupported settings %s" % (u, sorted(unknown)))
+        m = {**base, **kw}
+        row = dict(temperature=m["temperature"], top_k=m["top_k"], top_p=m["top_p"],
+                   repetition_penalty=m["repetition_penalty"],
+                   typical_mass=_typical_mass(m["typical_sampling"], m["typical_mass"]) if "typical_sampling" in m
+                   else None)
+        lib.sample_params_row(**row)
+        out.append(row)
+    return out
+
+
 def get_model_path(model_name, models_dir=MODELS_DIR):
     if model_name not in MODELS:
         raise ValueError(f"Model {model_name} not found in available models.")
@@ -284,7 +312,8 @@ class TextToSpeech:
         return wav.reshape(1, 1, -1), n
 
     # ------------------------------------------------------------------ several sentences per call
-    def tts_batch(self, texts, voice_samples=None, text_tokens_list=None, conditioning_latents_list=None, **kwargs):
+    def tts_batch(self, texts, voice_samples=None, text_tokens_list=None, conditioning_latents_list=None, kwargs_list=None,
+                  **kwargs):
         """Several sentences in one call, each ONE sequence: entry u of the returned list is what
         `tts(texts[u], voice_samples, **kwargs)` returns (fp32 [1, 1, samples] on the device). The conditioning latent
         and the seed are computed once, and every sentence samples with the uniforms row tts() draws from that seed.
@@ -298,12 +327,16 @@ class TextToSpeech:
         tts(texts[u], voice_samples=clips). It excludes `voice_samples`. `last_timings`: ar_ms
         (the decode batches, prefills included), prefill_ms (their prompt prefills), latents_ms and hifigan_ms (summed
         over the sentences), device_total_ms, and tokens (the tokens kept per sentence). Every rank computes the whole
-        batch, as tts() does."""
+        batch, as tts() does.
+        `kwargs_list`: one dict per text of sampling settings (temperature, top_p, top_k, repetition_penalty,
+        length_penalty, typical_sampling, typical_mass) over `kwargs`: entry u is then
+        `tts(texts[u], ..., **{**kwargs, **kwargs_list[u]})`. The rows of one decode batch sample with their own settings
+        (the per-row sampler); without kwargs_list every row shares the call's settings."""
         texts = list(texts)
         if not texts:
             raise ValueError("tts_batch needs at least one text")
         self._check_lists(texts, voice_samples, text_tokens_list, conditioning_latents_list)
-        return self._tts_batch(texts, voice_samples, text_tokens_list, conditioning_latents_list, **kwargs)
+        return self._tts_batch(texts, voice_samples, text_tokens_list, conditioning_latents_list, kwargs_list, **kwargs)
 
     @staticmethod
     def _check_lists(texts, voice_samples, text_tokens_list, conditioning_latents_list):
@@ -322,7 +355,8 @@ class TextToSpeech:
             return [c.to(self.device).float().reshape(-1) for c in conditioning_latents_list]
         return [self._auto_latent(voice_samples)] * n
 
-    def _tts_batch(self, texts, voice_samples, text_tokens_list, conditioning_latents_list, k=1, verbose=True, use_deterministic_seed=None,
+    def _tts_batch(self, texts, voice_samples, text_tokens_list, conditioning_latents_list, kwargs_list, k=1, verbose=True,
+                   use_deterministic_seed=None,
                    num_autoregressive_samples=512, temperature=.8, length_penalty=1, repetition_penalty=2.0, top_p=.8,
                    max_mel_tokens=500, cvvp_amount=.0, top_k=50, typical_sampling=False, typical_mass=.9,
                    **hf_generate_kwargs):
@@ -330,6 +364,10 @@ class TextToSpeech:
         if hf_generate_kwargs:
             raise TypeError(f"unsupported generate kwargs: {sorted(hf_generate_kwargs)}")
         typical = _typical_mass(typical_sampling, typical_mass)
+        settings = None if kwargs_list is None else row_settings(
+            kwargs_list, len(texts), dict(temperature=temperature, top_k=top_k, top_p=top_p,
+                                          repetition_penalty=repetition_penalty, length_penalty=length_penalty,
+                                          typical_sampling=typical_sampling, typical_mass=typical_mass), BATCH_SETTINGS)
         seed = self.deterministic_state(seed=use_deterministic_seed)
         toks = [self._inputs_tokens(texts[u], None if text_tokens_list is None else text_tokens_list[u])
                 for u in range(len(texts))]
@@ -359,11 +397,14 @@ class TextToSpeech:
                 if timed:
                     ev[0].record()
                 if len(batch) == 1:
+                    one = dec if settings is None else {**dec, **settings[batch[0]]}
                     codes = [ar.generate(autos[batch[0]], toks[batch[0]], 1, n_max, uniforms=uniforms,
-                                         prefill_events=pre, **dec)]
+                                         prefill_events=pre, **one)]
                 else:
+                    per_row = {} if settings is None else {"row_settings": [settings[u] for u in batch]}
                     codes = ar.generate_grouped([autos[u] for u in batch], [toks[u] for u in batch], [1] * len(batch),
-                                                n_max, uniforms_list=[uniforms] * len(batch), prefill_events=pre, **dec)
+                                                n_max, uniforms_list=[uniforms] * len(batch), prefill_events=pre,
+                                                **dec, **per_row)
                 if timed:
                     ev[3].record()
                     timed_parts.append((ev, [("ar_ms", 0, 3), ("prefill_ms", 1, 2)]))
@@ -398,7 +439,7 @@ class TextToSpeech:
 
     # ------------------------------------------------------------------ many streams per call
     def tts_stream_batch(self, texts, voice_samples=None, conditioning_latents_list=None, text_tokens_list=None,
-                         **kwargs):
+                         kwargs_list=None, **kwargs):
         """Streams several texts at once: a generator of `(u, chunk, last)`. For each u, the chunks arrive in the order
         `tts_stream(texts[u], ...)` yields them, with the same count and lengths; `last` marks the final chunk of stream
         u. Chunks of different streams interleave. Every text is one row of ONE grouped decode batch (at most
@@ -413,6 +454,9 @@ class TextToSpeech:
         `voice_samples`: one voice for all texts; `conditioning_latents_list`: one auto conditioning latent per text (as
         get_conditioning_latents returns it), not both. `text_tokens_list` (one id list per text) bypasses the
         tokenizer. The other keyword arguments are those of tts_stream, accepted and rejected as it does.
+        `kwargs_list`: one dict per text of temperature / top_p / top_k / repetition_penalty / length_penalty over the
+        other keyword arguments (another key raises TypeError): stream u is then that of `tts_stream(texts[u], ...,
+        **{**kwargs, **kwargs_list[u]})`, each row sampling with its own settings. The chunk size stays one for the batch.
         `last_timings` (set when the generator is exhausted): ar_ms (decode, prefills included), hifigan_ms,
         device_total_ms and tokens (per row)."""
         texts = list(texts)
@@ -428,9 +472,9 @@ class TextToSpeech:
             if len(t) + 4 > lib.AR_STEP_MAX_P:
                 raise ValueError("text %d: a prompt of %d positions (at most %d in a batch; tts_stream streams it alone)"
                                  % (u, len(t) + 4, lib.AR_STEP_MAX_P))
-        return self._stream_batch(toks, voice_samples, conditioning_latents_list, **kwargs)
+        return self._stream_batch(toks, voice_samples, conditioning_latents_list, kwargs_list, **kwargs)
 
-    def _stream_batch(self, toks, voice_samples, conditioning_latents_list, conditioning_latents=None, k=1,
+    def _stream_batch(self, toks, voice_samples, conditioning_latents_list, kwargs_list, conditioning_latents=None, k=1,
                       verbose=True, use_deterministic_seed=None, return_deterministic_state=False, overlap_wav_len=1024,
                       stream_chunk_size=40, num_autoregressive_samples=512, temperature=.8, length_penalty=1,
                       repetition_penalty=2.0, top_p=.8, max_mel_tokens=500, cvvp_amount=.0, diffusion_iterations=100,
@@ -439,6 +483,9 @@ class TextToSpeech:
         if hf_generate_kwargs:
             raise TypeError(f"unsupported generate kwargs: {sorted(hf_generate_kwargs)}")
         dec = dict(temperature=temperature, top_k=top_k, top_p=top_p, repetition_penalty=repetition_penalty)
+        if kwargs_list is not None:
+            dec["row_settings"] = row_settings(kwargs_list, len(toks), dict(dec, length_penalty=length_penalty),
+                                               STREAM_SETTINGS)
         return self._stream_batch_run(toks, voice_samples, conditioning_latents_list, verbose, use_deterministic_seed,
                                       overlap_wav_len, int(stream_chunk_size), dec)
 
@@ -515,7 +562,8 @@ class TextToSpeech:
                     cond_free=True, cond_free_k=2, diffusion_temperature=1.0, top_k=50, k=1, verbose=True,
                     num_autoregressive_samples=512, return_deterministic_state=False, **hf_generate_kwargs):
         """A StreamPool of `max_streams` (1..256) slots: texts submitted at any time stream from one running decode
-        batch. The keyword arguments are tts_stream's, accepted and rejected as it does; they apply to every stream."""
+        batch. The keyword arguments are tts_stream's, accepted and rejected as it does; they are every stream's
+        defaults, which StreamPool.submit may override per stream."""
         if hf_generate_kwargs:
             raise TypeError(f"unsupported generate kwargs: {sorted(hf_generate_kwargs)}")
         if not 1 <= int(max_streams) <= lib.AR_STEP_MAX_GROUPS:
@@ -565,6 +613,17 @@ class TextToSpeech:
                         pending[cur] = []
 
 
+def _whole(name, v):
+    """v as an int; ValueError unless it is a whole number."""
+    try:
+        i = int(v)
+    except (TypeError, ValueError):
+        raise ValueError("%s must be an integer, got %r" % (name, v)) from None
+    if isinstance(v, bool) or i != v:
+        raise ValueError("%s must be an integer, got %r" % (name, v))
+    return i
+
+
 class StreamPool:
     """Continuous batching of tts_stream: texts join a decode batch that is already running, each in a free slot, and
     leave it when they end. The chunks of stream `sid` are those of `tts_stream(text, voice_samples=...,
@@ -573,7 +632,10 @@ class StreamPool:
     steps (as in tts_stream_batch), so the samples agree with tts_stream's within rounding (DESIGN §5).
 
     Each stream has its own voice and seed: its uniforms row and its conditioning crop follow the seed as in tts_stream.
-    The sampling parameters belong to the pool (they are part of its step graph). A full pool queues texts first in,
+    Each stream may also have its own sampling settings, chunk size and cross-fade (`submit`); the pool's kwargs are
+    the defaults. The settings sit in a per-row table on the device. While every stream has the pool's settings the
+    decode samples with the scalar sampler, as before; the first stream with settings of its own switches the pool to
+    the per-row sampler (ttb_ar_sample_params), whose step graph is captured once, then. A full pool queues texts first in,
     first out; the pool looks at its queue at least every POOL_ADMIT_STEPS (16) decode steps, so a text starts decoding
     within 16 steps of a slot being free. `submit` may be called from any thread; every CUDA call happens on the thread
     that iterates the pool (`poll` / `run`). Every stream applies stream_flushes to its own token count and ends at its
@@ -586,7 +648,7 @@ class StreamPool:
 
     def __init__(self, tts, max_streams, overlap_wav_len, flush_every, dec):
         self.tts, self.capacity = tts, max_streams
-        self.overlap, self.flush_every = overlap_wav_len, flush_every
+        self.overlap, self.flush_every, self.dec = overlap_wav_len, flush_every, dec
         self.timed = tts.device.type == "cuda"
         self.ws = tts.autoregressive.slot_workspace(max_streams, STREAM_MAX_LENGTH, pos_mode=tts._pos_mode(),
                                                     use_graph=self.timed, **dec)
@@ -598,12 +660,23 @@ class StreamPool:
         self._closed = False
         self._ar_pending = []                          # (start, end, streams running) of decode steps not yet read
 
-    def submit(self, text, voice_samples=None, conditioning_latent=None, text_tokens=None, use_deterministic_seed=None):
+    def submit(self, text, voice_samples=None, conditioning_latent=None, text_tokens=None, use_deterministic_seed=None,
+               temperature=None, top_p=None, top_k=None, repetition_penalty=None, length_penalty=None,
+               stream_chunk_size=None, overlap_wav_len=None):
         """Queues a text; returns its stream id. `conditioning_latent` (an auto latent as get_conditioning_latents
         returns it) excludes `voice_samples`; neither = a random voice, as in tts_stream. A prompt longer than 352
-        positions raises ValueError (tts_stream can stream it alone)."""
+        positions raises ValueError (tts_stream can stream it alone).
+        temperature, top_p, top_k, repetition_penalty, stream_chunk_size and overlap_wav_len: this stream's own, as
+        tts_stream takes them; None = the pool's. length_penalty is accepted and has no effect, as in tts_stream. The
+        stream's chunks are then those of tts_stream(text, ..., **{**the pool's kwargs, **these}). A bad value raises
+        ValueError here, before anything is queued."""
         if voice_samples is not None and conditioning_latent is not None:
             raise ValueError("give voice_samples or conditioning_latent, not both")
+        given = dict(temperature=temperature, top_p=top_p, top_k=top_k, repetition_penalty=repetition_penalty)
+        settings = {k: v for k, v in given.items() if v is not None}
+        lib.sample_params_row(**{**self.dec, **settings})
+        every = self.flush_every if stream_chunk_size is None else _whole("stream_chunk_size", stream_chunk_size)
+        overlap = self.overlap if overlap_wav_len is None else _whole("overlap_wav_len", overlap_wav_len)
         toks = self.tts._inputs_tokens(text, text_tokens)
         if len(toks) + 4 > lib.AR_STEP_MAX_P:
             raise ValueError("a prompt of %d positions (a pool slot holds %d; tts_stream streams it alone)" %
@@ -614,7 +687,8 @@ class StreamPool:
             sid = self._next_sid
             self._next_sid += 1
             self._queue.append(dict(sid=sid, toks=toks, voice=voice_samples, cond=conditioning_latent,
-                                    seed=use_deterministic_seed, t_submit=perf_counter()))
+                                    seed=use_deterministic_seed, settings=settings, every=every, overlap=overlap,
+                                    t_submit=perf_counter()))
         return sid
 
     def _event(self):
@@ -642,10 +716,10 @@ class StreamPool:
             tts._auto_latent(rec["voice"])
         P = len(rec["toks"]) + 4
         cap = STREAM_MAX_LENGTH - P
-        every = self.flush_every
+        every = rec["every"]
         first = max(every, FIRST_BUFFER) if every > 0 else cap
         e0 = self._event()
-        self.ws.admit(slot, auto, rec["toks"], tts._uniforms(seed, cap))
+        self.ws.admit(slot, auto, rec["toks"], tts._uniforms(seed, cap), rec["settings"])
         e1 = self._event()
         rec.update(auto=auto, cap=cap, block=every if every > 0 else cap, obs=min(first, cap), flushed=0,
                    wav_prev=None, wav_tail=None, t_admit=perf_counter(), t_first=None, prefill=(e0, e1),
@@ -696,7 +770,7 @@ class StreamPool:
                 n, ended = int(hit[0].item()) + 1, True
             else:
                 n, ended = h, h >= rec["cap"]
-            flags = stream_flushes(n, rec["flushed"], ended, self.flush_every)
+            flags = stream_flushes(n, rec["flushed"], ended, rec["every"])
             if flags:
                 jobs.setdefault(n, []).append((s, flags))
             if ended:
@@ -718,7 +792,7 @@ class StreamPool:
                     # tts_stream decodes every flush into a buffer of its own, and handle_chunks fades in place
                     w = wav_gen if i == 0 else wav_gen.clone()
                     chunk, rec["wav_prev"], rec["wav_tail"] = self.tts.handle_chunks(w, rec["wav_prev"], rec["wav_tail"],
-                                                                                      self.overlap)
+                                                                                      rec["overlap"])
                     rec["flushed"] = n
                     if rec["t_first"] is None:
                         rec["t_first"] = perf_counter()

@@ -223,6 +223,10 @@ class AREngine:
         # ---- decode workspaces: one per chain (contiguous candidate ranges)
         per = B // nch
         st["chains"] = [self._chain_state(st, per, c * per, compact=nch > 1) for c in range(nch)]
+        # the per-row sampling settings (include/ttb.h TtbSampleParams, 8 words a row) read by a per-row decode
+        st["params"] = torch.zeros(B, 8, dtype=torch.int32, device=dev)
+        for ch in st["chains"]:
+            ch["params"] = st["params"][ch["b0"]: ch["b0"] + ch["B"]]
         st["sides"] = [torch.cuda.Stream(device=dev) for _ in range(nch - 1)] if dev.type == "cuda" else []
         st["graph"] = None
         st["graph_params"] = None
@@ -366,8 +370,13 @@ class AREngine:
 
     def _sample(self, sp, logits, ld_logits, ch):
         """The sampler over the logits of one chain (ld_logits = 0: row 0 for every candidate); the typical-set entry
-        when `sp` turns the filter on."""
+        when `sp` turns the filter on, the per-row entry (each row's settings from ch["params"]) when `sp` is per-row."""
         Nmax = ch["Nmax"]
+        if sp.get("per_row"):
+            lib.ar_sample_params(logits, ld_logits, self.V, ch["B"], ch["uniforms"], Nmax, ch["seen"], ch["codes"], Nmax,
+                                 ch["finished"], ch["state"], ch["params"], self.cfg.stop_mel_token, advance=True,
+                                 **_rows(ch))
+            return
         args = (logits, ld_logits, self.V, ch["B"], ch["uniforms"], Nmax, ch["seen"], ch["codes"], Nmax, ch["finished"],
                 ch["state"], sp["temperature"], sp["top_k"], sp["top_p"], sp["rep_penalty"], self.cfg.stop_mel_token)
         if sp.get("typical_mass") is None:
@@ -418,11 +427,12 @@ class AREngine:
         ch["seen"][rows, w] |= (1 << bit) if bit < 31 else -(1 << 31)
 
     def _begin_grouped(self, cond_latent, text_tokens_list, counts, Nmax, uniforms_list, seed, sp, trace_logits=None,
-                       prefill_events=None):
+                       prefill_events=None, params=None):
         """_begin for a batch of utterances: one prefill per utterance into its own prefix, and the first token of every
         row sampled from its utterance's prefill logits (one sampler call per chain, so the step counter advances once).
         `cond_latent`: one conditioning latent for every utterance, or a list with one per utterance.
-        `prefill_events`: None or a pair of CUDA events recorded around the prefills."""
+        `prefill_events`: None or a pair of CUDA events recorded around the prefills. `params`: the per-row settings
+        table (lib.sample_params_table, one row per decode row) of a per-row `sp`, written before the first token."""
         dev = self.dev
         conds = list(cond_latent) if isinstance(cond_latent, (list, tuple)) else [cond_latent] * len(counts)
         if len(conds) != len(counts):
@@ -437,6 +447,8 @@ class AREngine:
                 u = torch.rand(n, Nmax, generator=g, device=dev)
             us.append(u.to(device=dev, dtype=torch.float32))
         uniforms = torch.cat(us, dim=0)
+        if params is not None:
+            st["params"].copy_(params)
         if prefill_events is not None:
             prefill_events[0].record()
         for gs, cond, toks in zip(st["groups"], conds, text_tokens_list):
@@ -497,15 +509,20 @@ class AREngine:
         return cs[0].clone() if len(cs) == 1 else torch.cat(cs, dim=0)
 
     @staticmethod
-    def _sampling(temperature, top_k, top_p, repetition_penalty, pos_mode, typical_mass=None, capture=False):
+    def _sampling(temperature, top_k, top_p, repetition_penalty, pos_mode, typical_mass=None, capture=False,
+                  per_row=False):
         """The sampling parameters of a decode; also the key of the captured step graph, so a change of any of them
         (the typical mass and the latent capture included) captures a new graph. typical_mass None = no typical filter.
         capture: every step ends with ttb_ar_capture_latents into each chain's ch["lat"]; without it the step (and its
-        graph) is what it is without this option."""
+        graph) is what it is without this option. per_row: the sampler reads every row's settings from the decode
+        state's table st["params"] (ttb_ar_sample_params), which is not part of the key: new settings in the table reuse
+        the graph, and the scalar settings here are unused."""
         sp = dict(temperature=float(temperature), top_k=int(top_k), top_p=float(top_p),
                   rep_penalty=float(repetition_penalty), pos_mode=1 if pos_mode == "ref_kv_quirk" else 0)
         if capture:
             sp["capture"] = True
+        if per_row:
+            sp["per_row"] = True
         if typical_mass is not None:
             m = float(typical_mass)
             if not 0.0 < m <= 1.0:
@@ -533,26 +550,48 @@ class AREngine:
     def generate_grouped(self, cond_latent, text_tokens_list, counts, max_new, uniforms_list=None, seed=None,
                          temperature=0.8, top_k=50, top_p=0.8, repetition_penalty=2.0, pos_mode="ref_kv_quirk",
                          use_graph=True, stop_check_every=32, trace_logits=None, typical_mass=None,
-                         prefill_events=None):
+                         prefill_events=None, row_settings=None):
         """Several utterances decoded in ONE batch: utterance u contributes counts[u] candidates that attend to its own
         prompt (text_tokens_list[u]; `cond_latent` is one conditioning latent for all, or a list with one per utterance,
         each utterance's latent then starting its own prompt). Returns one int32 codes tensor [counts[u], max_new]
         per utterance, each as generate(cond_latent, text_tokens_list[u], counts[u], max_new, uniforms_list[u], ...)
         returns it. At most lib.AR_STEP_MAX_GROUPS utterances, lib.AR_STEP_MAX_B rows and prompts of
         lib.AR_STEP_MAX_P positions (plan_batches packs within these limits); the one-kernel step is required.
-        `prefill_events`: None or a pair of CUDA events recorded around the prefills."""
+        `prefill_events`: None or a pair of CUDA events recorded around the prefills. `row_settings`: None, or one dict
+        per utterance of sampling settings (keys temperature, top_k, top_p, repetition_penalty, typical_mass; a missing
+        key takes the argument of this call) for all of its rows: utterance u then samples as generate(...) with its
+        settings, through the per-row sampler."""
         counts = [int(n) for n in counts]
         if len(counts) != len(text_tokens_list) or (uniforms_list is not None and len(uniforms_list) != len(counts)):
             raise ValueError("one entry of counts (and of uniforms_list) per utterance")
         Nmax = int(max_new)
-        sp = self._sampling(temperature, top_k, top_p, repetition_penalty, pos_mode, typical_mass)
+        params = self._row_params(row_settings, counts, temperature, top_k, top_p, repetition_penalty, typical_mass)
+        sp = self._sampling(temperature, top_k, top_p, repetition_penalty, pos_mode,
+                            typical_mass if params is None else None, per_row=params is not None)
         if trace_logits is not None:
             use_graph = False
         st = self._begin_grouped(cond_latent, text_tokens_list, counts, Nmax, uniforms_list, seed, sp, trace_logits,
-                                 prefill_events)
+                                 prefill_events, params)
         self._decode(st, sp, Nmax - 1, use_graph, stop_check_every, trace_logits)
         codes = self._codes(st)
         return [codes[g["b0"]: g["b1"]].clone() for g in st["groups"]]
+
+    def _row_params(self, row_settings, counts, temperature, top_k, top_p, repetition_penalty, typical_mass):
+        """The per-row settings table of a grouped decode (lib.sample_params_table, validated) from one settings dict
+        per group, each expanded to its group's rows over the call's own settings; None without row_settings."""
+        if row_settings is None:
+            return None
+        if len(row_settings) != len(counts):
+            raise ValueError("%d row_settings for %d utterances" % (len(row_settings), len(counts)))
+        base = dict(temperature=temperature, top_k=top_k, top_p=top_p, repetition_penalty=repetition_penalty,
+                    typical_mass=typical_mass)
+        rows = []
+        for n, rs in zip(counts, row_settings):
+            unknown = set(rs) - set(base)
+            if unknown:
+                raise TypeError("unknown sampling settings: %s" % sorted(unknown))
+            rows += [{**base, **rs}] * n
+        return lib.sample_params_table(rows, self.dev)
 
     def _decode(self, st, sp, steps, use_graph, stop_check_every, trace_logits):
         """The decode loop after the first token: `steps` steps (graph replays polled for the stop every
@@ -619,7 +658,7 @@ class AREngine:
 
     def generate_grouped_stream(self, cond_latent, text_tokens_list, max_new, first_block, block, uniforms_list=None,
                                 seed=None, temperature=0.8, top_k=50, top_p=0.8, repetition_penalty=2.0,
-                                pos_mode="ref_kv_quirk", use_graph=True, typical_mass=None):
+                                pos_mode="ref_kv_quirk", use_graph=True, typical_mass=None, row_settings=None):
         """generate_stream for several utterances, ONE row each, decoded in one grouped batch (limits of
         generate_grouped); each row attends to its own prompt text_tokens_list[u], after its own conditioning latent
         (`cond_latent`: one for all, or a list). `max_new`: the cap of every row, or a list with one per row; the batch
@@ -630,7 +669,8 @@ class AREngine:
         every row has ended: codes[u] = int32 [n_u] the tokens of row u so far, ended[u] as generate_stream decides it
         for that row alone (its stop token, kept as the last element, or its cap reached); a row that has ended keeps
         its last codes in later yields. `latents` fp32 [rows, max(max_new), D]: latents[u, i] belongs to codes[u][i];
-        the buffer belongs to the decode workspace and stays valid until the next decode."""
+        the buffer belongs to the decode workspace and stays valid until the next decode. `row_settings`: one
+        sampling-settings dict per row, as for generate_grouped."""
         n = len(text_tokens_list)
         caps = [int(m) for m in max_new] if isinstance(max_new, (list, tuple)) else [int(max_new)] * n
         if len(caps) != n or min(caps) < 1:
@@ -646,8 +686,10 @@ class AREngine:
                 if u.shape[1] < c:
                     raise ValueError("uniforms of %d steps for a cap of %d" % (u.shape[1], c))
                 us.append(torch.nn.functional.pad(u[:, :Nmax], (0, max(0, Nmax - u.shape[1]))))
-        sp = self._sampling(temperature, top_k, top_p, repetition_penalty, pos_mode, typical_mass, capture=True)
-        st = self._begin_grouped(cond_latent, text_tokens_list, [1] * n, Nmax, us, seed, sp)
+        params = self._row_params(row_settings, [1] * n, temperature, top_k, top_p, repetition_penalty, typical_mass)
+        sp = self._sampling(temperature, top_k, top_p, repetition_penalty, pos_mode,
+                            typical_mass if params is None else None, capture=True, per_row=params is not None)
+        st = self._begin_grouped(cond_latent, text_tokens_list, [1] * n, Nmax, us, seed, sp, params=params)
         if "lat" not in st:
             st["lat"] = torch.empty(n, Nmax, D, dtype=torch.float32, device=self.dev)
         lat = st["lat"]
@@ -694,9 +736,11 @@ class AREngine:
 
     def slot_workspace(self, capacity, max_new, temperature=0.8, top_k=50, top_p=0.8, repetition_penalty=2.0,
                        pos_mode="ref_kv_quirk", use_graph=True):
-        """A decode workspace of `capacity` one-row slots that rows join and leave while it runs (SlotWorkspace)."""
+        """A decode workspace of `capacity` one-row slots that rows join and leave while it runs (SlotWorkspace). The
+        sampling settings are the default of every row; SlotWorkspace.admit may give a row its own."""
+        defaults = dict(temperature=temperature, top_k=top_k, top_p=top_p, repetition_penalty=repetition_penalty)
         return SlotWorkspace(self, capacity, max_new, self._sampling(temperature, top_k, top_p, repetition_penalty,
-                                                                     pos_mode, capture=True), use_graph)
+                                                                     pos_mode, capture=True), use_graph, defaults)
 
     # ------------------------------------------------------------------ teacher-forced passes
     def _forward_sequences(self, emb_fn, nseq, T):
@@ -810,9 +854,13 @@ class SlotWorkspace:
     the shared step counter reads s has row_start s - 1, so it samples exactly the tokens that a decode of its own from
     step 0 samples. Every step captures the latents (ttb_ar_capture_latents_rows). The step forms are those of the
     grouped decode (fused up to FUSED_MAX_B rows, mixed, two chains from CHAINS_MIN_B rows); the per-op form has no
-    groups and raises. All calls enqueue on the current CUDA stream."""
+    groups and raises. A row may sample with its own settings: `admit` writes them into the slot's entry of the
+    settings table (st["params"]). While every row has the workspace's settings, the step samples with the scalar
+    sampler, as a workspace without per-row settings does. The first row admitted with other settings switches the
+    workspace to the per-row sampler (ttb_ar_sample_params, one new step graph, captured then); from there on rows with
+    any settings join without another capture. All calls enqueue on the current CUDA stream."""
 
-    def __init__(self, eng, capacity, max_new, sp, use_graph=True):
+    def __init__(self, eng, capacity, max_new, sp, use_graph=True, defaults=None):
         capacity, Nmax = int(capacity), int(max_new)
         if not 1 <= capacity <= lib.AR_STEP_MAX_GROUPS:
             raise ValueError("a slot workspace has 1..%d slots, got %d" % (lib.AR_STEP_MAX_GROUPS, capacity))
@@ -820,6 +868,8 @@ class SlotWorkspace:
         if eng.MODE == "perop" or not lib.ar_step_supported(capacity, eng.D, eng.H, Pcap):
             raise lib.TtbError("a slot workspace needs the one-kernel step (mode %s)" % eng.MODE)
         self.eng, self.sp, self.capacity, self.Nmax, self.P_cap = eng, sp, capacity, Nmax, Pcap
+        self.defaults = dict(defaults or {})
+        self._default_words = lib.sample_params_row(**self.defaults)
         self.use_graph = use_graph and eng.dev.type == "cuda"
         dev, D = eng.dev, eng.D
         st = eng._build_state(("slots", capacity, Nmax), capacity, None, Nmax, [1] * capacity, [Pcap] * capacity,
@@ -829,6 +879,7 @@ class SlotWorkspace:
             gs["pkv"].zero_()
         st["row_start"] = torch.zeros(capacity, dtype=torch.int32, device=dev)
         st["lat"] = torch.zeros(capacity, Nmax, D, dtype=torch.float32, device=dev)
+        st["params"].copy_(torch.tensor(self._default_words, dtype=torch.int32).expand(capacity, -1))
         self.where = []                       # slot -> (chain, row in the chain)
         for ch in st["chains"]:
             ch["row_start"] = st["row_start"][ch["b0"]: ch["b0"] + ch["B"]]
@@ -846,18 +897,29 @@ class SlotWorkspace:
         if self.use_graph:
             eng._ensure_graph(st, sp)
 
-    def admit(self, slot, cond_latent, text_tokens, uniforms_row):
-        """Starts a row in the free slot `slot`: prompt prefill into the slot's prefix, the slot's P in the step's group
-        table, its sampler state (as _reset_chain), latent 0, its row_start, and its first token, sampled from the
-        prefill logits with a scratch counter at 0 (the shared counter does not move). uniforms_row: [n] with
-        n <= max_new. Returns the prompt length P."""
+    def admit(self, slot, cond_latent, text_tokens, uniforms_row, settings=None):
+        """Starts a row in the free slot `slot`: its sampling settings in the slot's entry of the settings table,
+        prompt prefill into the slot's prefix, the slot's P in the step's group table, its sampler state (as
+        _reset_chain), latent 0, its row_start, and its first token, sampled from the prefill logits with the slot's
+        settings and a scratch counter at 0 (the shared counter does not move). uniforms_row: [n] with n <= max_new.
+        `settings`: a dict of temperature / top_k / top_p / repetition_penalty over the workspace's defaults (ValueError
+        for a bad value, before anything is enqueued); settings other than the defaults switch the workspace to the
+        per-row sampler if it is not there yet. Returns the prompt length P."""
         eng, sp = self.eng, self.sp
         if self.live[slot]:
             raise ValueError("slot %d is in use" % slot)
         P = len(text_tokens) + 4
         if P > self.P_cap:
             raise ValueError("a prompt of %d positions (a slot holds %d)" % (P, self.P_cap))
+        unknown = set(settings or {}) - set(self.defaults)
+        if unknown:
+            raise TypeError("unknown sampling settings: %s" % sorted(unknown))
+        words = lib.sample_params_row(**{**self.defaults, **(settings or {})})
+        if words != self._default_words and not self.sp.get("per_row"):
+            self._use_per_row()
+            sp = self.sp
         ch, r = self.where[slot]
+        ch["params"][r].copy_(torch.tensor(words, dtype=torch.int32))
         gs = self.st["groups"][slot]
         eng._prefill(cond_latent, text_tokens, gs)
         eng._step_handle(ch, sp["pos_mode"]).set_group_len(r, P)
@@ -870,11 +932,22 @@ class SlotWorkspace:
         self.rs[slot] = self.step - 1
         self._first_state.zero_()
         Nmax = self.Nmax
-        lib.ar_sample(gs["logits"], eng.V, eng.V, 1, ch["uniforms"][r:r + 1], Nmax, ch["seen"][r:r + 1],
-                      ch["codes"][r:r + 1], Nmax, ch["finished"][r:r + 1], self._first_state, sp["temperature"],
-                      sp["top_k"], sp["top_p"], sp["rep_penalty"], eng.cfg.stop_mel_token, advance=False)
+        args = (gs["logits"], eng.V, eng.V, 1, ch["uniforms"][r:r + 1], Nmax, ch["seen"][r:r + 1], ch["codes"][r:r + 1],
+                Nmax, ch["finished"][r:r + 1], self._first_state)
+        if sp.get("per_row"):
+            lib.ar_sample_params(*args, ch["params"][r:r + 1], eng.cfg.stop_mel_token, advance=False)
+        else:
+            lib.ar_sample(*args, sp["temperature"], sp["top_k"], sp["top_p"], sp["rep_penalty"], eng.cfg.stop_mel_token,
+                          advance=False)
         self.live[slot] = True
         return P
+
+    def _use_per_row(self):
+        """Switches the step to the per-row sampler (every row's entry of st["params"] already holds its settings) and
+        captures its graph; called between steps, on a free slot's admission."""
+        self.sp = dict(self.sp, per_row=True)
+        if self.use_graph:
+            self.eng._ensure_graph(self.st, self.sp)
 
     def release(self, slot):
         """Frees a slot: its row stops sampling, and from the next advance on it is re-based every time so that it

@@ -3,7 +3,9 @@
 There is NO fallback: if the library is missing or a call fails, this module raises.
 """
 import ctypes as C
+import math
 import os
+import struct
 
 import torch
 
@@ -82,7 +84,7 @@ SYMBOLS = [
     "ttb_pair_exchange", "ttb_enable_peer_access", "ttb_peer_alloc", "ttb_peer_open", "ttb_peer_close", "ttb_peer_free",
     "ttb_wav2vec_conv0", "ttb_layernorm_act", "ttb_argmax_rows", "ttb_ar_sample_typical", "ttb_ar_capture_latents",
     "ttb_ar_embed_step_rows", "ttb_ar_sample_rows", "ttb_ar_capture_latents_rows", "ttb_ar_step_store_prefix_cap",
-    "ttb_ar_step_set_group_len",
+    "ttb_ar_step_set_group_len", "ttb_ar_sample_params",
 ]
 
 
@@ -330,6 +332,60 @@ def ar_sample_typical(logits, ld_logits, V, B, uniforms, ld_u, seen, codes, ld_c
                                       ld_codes, _p(finished), _p(state), C.c_float(temperature), top_k, C.c_float(top_p),
                                       C.c_float(rep_penalty), stop_token, 1 if advance else 0, C.c_float(typical_mass),
                                       _stream()), "ttb_ar_sample_typical")
+
+
+def ar_sample_params(logits, ld_logits, V, B, uniforms, ld_u, seen, codes, ld_codes, finished, state, params, stop_token,
+                     advance=True, row_start=None):
+    """ar_sample with row b's settings read from params[b] (a sample_params_table; include/ttb.h ttb_ar_sample_params).
+    `row_start`: per-row start steps, as for ar_sample."""
+    assert params.dtype == torch.int32 and params.dim() == 2 and params.shape[1] == 8 and params.shape[0] >= B, \
+        (params.dtype, params.shape)
+    _chk(load().ttb_ar_sample_params(_p(_f32(logits)), ld_logits, V, B, _p(_f32(uniforms)), ld_u, _p(seen), _p(codes),
+                                     ld_codes, _p(finished), _p(state), _p(params), stop_token, 1 if advance else 0,
+                                     _p(row_start), _stream()), "ttb_ar_sample_params")
+
+
+SAMPLE_TOP_K_MAX = 50      # the sampler's candidate arrays (csrc/ar.cu SAMP_CAP) hold the top 50 and their ties
+
+
+def sample_params_row(temperature=0.8, top_k=50, top_p=0.8, repetition_penalty=2.0, typical_mass=None):
+    """One row's sampling settings, validated (ValueError for a bad value), as the 8 int32 words of a TtbSampleParams
+    (include/ttb.h). typical_mass None = no typical filter (stored as 0)."""
+    def real(name, v):
+        try:
+            f = float(v)
+        except (TypeError, ValueError):
+            raise ValueError("%s must be a number, got %r" % (name, v)) from None
+        if isinstance(v, bool) or not math.isfinite(f):
+            raise ValueError("%s must be a finite number, got %r" % (name, v))
+        return f
+    t = real("temperature", temperature)
+    if not t > 0.0:
+        raise ValueError("temperature must be > 0, got %r" % (temperature,))
+    k = real("top_k", top_k)
+    if k != int(k) or not 1 <= k <= SAMPLE_TOP_K_MAX:
+        raise ValueError("top_k must be an integer in 1..%d, got %r" % (SAMPLE_TOP_K_MAX, top_k))
+    k = int(k)
+    p = real("top_p", top_p)
+    if not 0.0 < p <= 1.0:
+        raise ValueError("top_p must lie in (0, 1], got %r" % (top_p,))
+    r = real("repetition_penalty", repetition_penalty)
+    if not r > 0.0:
+        raise ValueError("repetition_penalty must be > 0, got %r" % (repetition_penalty,))
+    m = 0.0
+    if typical_mass is not None:
+        m = real("typical_mass", typical_mass)
+        if not 0.0 < m <= 1.0:
+            raise ValueError("typical_mass must lie in (0, 1], got %r" % (typical_mass,))
+    words = struct.unpack("4i", struct.pack("4f", t, p, r, m))
+    return list(words) + [k, 0, 0, 0]
+
+
+def sample_params_table(rows, device):
+    """The TtbSampleParams table [len(rows)] of a batch as a device int32 tensor [len(rows), 8]: rows[b] is a dict of
+    sample_params_row's keyword arguments. Every row is validated before anything is allocated."""
+    words = [sample_params_row(**r) for r in rows]
+    return torch.tensor(words, dtype=torch.int32).to(device)
 
 
 def ar_capture_latents(x, B, D, g1, b1, g2, b2, state, Nmax, out, ld_row, row_start=None):
