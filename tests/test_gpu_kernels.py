@@ -266,35 +266,52 @@ def test_fix_codes():
 
 
 def test_diffusion_step_kernel():
+    """ttb_diffusion_step at the first, a middle and the last call, with and without classifier-free guidance. `parity`
+    lays model_out out as the double-buffered peer-exchange area (parity_stride) of the two-GPU CFG pair, with the other
+    slot holding garbage. The bf16 copy leaves columns C..ld_xb-1 alone, and the mel is written at the last call (i == 0)
+    only."""
     from tortoise_tts_b200 import lib
     from tortoise_tts_b200.diffusion_engine import make_schedule
     torch.manual_seed(6)
-    S, C, iters = 50, 100, 7
+    S, C, iters, ld_xb = 50, 100, 7, 128
     tmap, tables = make_schedule(iters)
     tb = torch.from_numpy(tables).cuda()
-    for call in (0, 3, 6):
-        i = iters - 1 - call
-        mo = torch.randn(2, S, 2 * C, device="cuda")
-        x = torch.randn(S, C, device="cuda")
-        x0 = x.clone()
-        noise = torch.randn(iters, S, C, device="cuda")
-        xb = torch.zeros(S, 128, device="cuda", dtype=torch.bfloat16)
-        step = torch.tensor([call], dtype=torch.int32, device="cuda")
-        mel = torch.zeros(C, S, device="cuda")
-        lib.diffusion_step(mo, S * 2 * C, 2 * C, x, xb, 128, noise, tb, step, S, C, iters, True, 2.0, mel)
-        eps, var = mo[0, :, :C], mo[0, :, C:]
-        cfk = 2.0 * (1 - i / iters)
-        eps = (1 + cfk) * eps - cfk * mo[1, :, :C]
-        frac = (var + 1) / 2
-        logvar = frac * tb[3, i] + (1 - frac) * tb[2, i]
-        xs = (tb[0, i] * x0 - tb[1, i] * eps).clamp(-1, 1)
-        mean = tb[4, i] * xs + tb[5, i] * x0
-        want = mean + (0.0 if i == 0 else 1.0) * torch.exp(0.5 * logvar) * noise[call]
-        assert (x - want).abs().max().item() < 1e-4
-        assert (xb[:, :C].float() - want).abs().max().item() < 0.05
-        if i == 0:
-            wm = ((want + 1) / 2) * (2.3143386840820312 + 11.512925148010254) - 11.512925148010254
-            assert (mel - wm.t()).abs().max().item() < 1e-3
+    n = S * 2 * C
+    for cond_free, parity in ((True, False), (False, False), (True, True), (False, True)):
+        for call in (0, 3, 6):
+            i = iters - 1 - call
+            mo = torch.randn(2, S, 2 * C, device="cuda")
+            if parity:
+                area = torch.full((2, 2 * n), float("nan"), device="cuda")
+                area[call & 1] = mo.reshape(-1)
+                model_out, stride = area, 2 * n
+            else:
+                model_out, stride = mo, 0
+            x = torch.randn(S, C, device="cuda")
+            x0 = x.clone()
+            noise = torch.randn(iters, S, C, device="cuda")
+            xb = torch.full((S, ld_xb), float("nan"), device="cuda", dtype=torch.bfloat16)
+            step = torch.tensor([call], dtype=torch.int32, device="cuda")
+            mel = torch.full((C, S), float("nan"), device="cuda")
+            lib.diffusion_step(model_out, n, 2 * C, x, xb, ld_xb, noise, tb, step, S, C, iters, cond_free, 2.0, mel,
+                               parity_stride=stride)
+            eps, var = mo[0, :, :C], mo[0, :, C:]
+            if cond_free:
+                cfk = 2.0 * (1 - i / iters)
+                eps = (1 + cfk) * eps - cfk * mo[1, :, :C]
+            frac = (var + 1) / 2
+            logvar = frac * tb[3, i] + (1 - frac) * tb[2, i]
+            xs = (tb[0, i] * x0 - tb[1, i] * eps).clamp(-1, 1)
+            mean = tb[4, i] * xs + tb[5, i] * x0
+            want = mean + (0.0 if i == 0 else 1.0) * torch.exp(0.5 * logvar) * noise[call]
+            assert (x - want).abs().max().item() < 1e-4
+            assert torch.equal(xb[:, :C], x.to(torch.bfloat16))
+            assert torch.isnan(xb[:, C:].float()).all()
+            if i == 0:
+                wm = ((want + 1) / 2) * (2.3143386840820312 + 11.512925148010254) - 11.512925148010254
+                assert (mel - wm.t()).abs().max().item() < 1e-3
+            else:
+                assert torch.isnan(mel).all()
 
 
 def test_vocoder_convs():
