@@ -332,6 +332,13 @@ int ttb_diffusion_step(const TtbDiffStepArgs* args, void* stream);
  * learned-variance half of model_out is not read. `noise` may be NULL when every sigma is 0 (eta = 0). x_bf16, mel_out
  * and parity_stride act as in the p_sample epilogue above. */
 int ttb_ddim_step(const TtbDiffStepArgs* args, void* stream);
+/* DPM-Solver++(2M) epilogue (Lu et al. 2022, arXiv:2211.01095, Algorithm 2; no reference counterpart) on the same
+ * arguments, with another meaning of `tables`: fp32 [6, iters] rows sqrt_recip_ac, sqrt_recipm1_ac, a, b, w, w_p
+ * (diffusion_engine.make_dpmpp2m_schedule). Per element: the same CFG mix, D = clamp(sqrt_recip_ac*x - sqrt_recipm1_ac*eps,
+ * -1, 1), x' = a*x + b*(w*D + w_p*x0_prev), then x0_prev = D. x0_prev (fp32 [S, C], required) is not read where w_p = 0
+ * (the first and the last call), so its contents before the first call do not matter. `noise` is not read and the
+ * learned-variance half of model_out is not read. x_bf16, mel_out and parity_stride act as in the p_sample epilogue. */
+int ttb_dpmpp2m_step(const TtbDiffStepArgs* args, float* x0_prev, void* stream);
 /* CFG branch pair on two GPUs (no reference counterpart: the reference runs both branches on one device,
  * utils/diffusion.py:340-342): copies this rank's branch output `src` (n floats) into slot (call & 1, branch_off) of the
  * local AND the partner's exchange area (peer memory mapped through CUDA IPC), publishes epoch + call + 1 in the

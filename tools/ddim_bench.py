@@ -1,9 +1,11 @@
-"""Device time of the diffusion stage with the p sampler and with DDIM, on one GPU, with CUDA events.
+"""Device time of the diffusion stage with the p sampler, with DDIM and with DPM-Solver++(2M), on one GPU, with CUDA
+events.
 
 The stage is DiffusionEngine.sample as tts() runs it (timestep-independent conditioning, tables, noise upload and every
 captured step, both CFG branches) on the full-size synthetic checkpoint at S = 1872 (430 latents, the length of the
-standard benchmark's utterance): p at 200 steps, DDIM (eta = 0) at 200, 100, 50 and 25 steps. Every arm is captured and
-warmed first; the timed rounds alternate the arms. The SM clock is read while the last round runs.
+standard benchmark's utterance): p at 200 steps, DDIM (eta = 0) at 200, 100, 50 and 25 steps, DPM-Solver++(2M) at 50,
+25, 20 and 10 steps. Every arm is captured and warmed first; the timed rounds alternate the arms. The SM clock is read
+while the last round runs.
 
 Prints one JSON line with the GPU's name, power limit and SM clock. Needs a CUDA device (there is no CPU fallback)."""
 import json
@@ -16,7 +18,8 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-ARMS = [("p", 200), ("ddim", 200), ("ddim", 100), ("ddim", 50), ("ddim", 25)]
+ARMS = [("p", 200), ("ddim", 200), ("ddim", 100), ("ddim", 50), ("ddim", 25),
+        ("dpm++2m", 50), ("dpm++2m", 25), ("dpm++2m", 20), ("dpm++2m", 10)]
 QUERY = ["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"]
 
 

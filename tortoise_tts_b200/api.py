@@ -162,18 +162,23 @@ def _typical_mass(typical_sampling, typical_mass):
     return m
 
 
-DIFFUSION_SAMPLERS = ("p", "ddim")
+DIFFUSION_SAMPLERS = ("p", "ddim", "dpm++2m")
 
 
 def _sampler_kwargs(diffusion_sampler, ddim_eta):
     """DiffusionEngine.sample kwargs for the tts() kwargs `diffusion_sampler` / `ddim_eta`. An unknown sampler or an eta
-    outside [0, 1] raises ValueError. The default sampler adds no kwargs, so its call is exactly the p-sampler call."""
+    outside [0, 1] raises ValueError (also where the sampler ignores eta). The default sampler adds no kwargs, so its call
+    is exactly the p-sampler call; only DDIM is given eta."""
     if diffusion_sampler not in DIFFUSION_SAMPLERS:
         raise ValueError("diffusion_sampler must be one of %s, got %r" % (DIFFUSION_SAMPLERS, diffusion_sampler))
     eta = float(ddim_eta)
     if not 0.0 <= eta <= 1.0:
         raise ValueError("ddim_eta must lie in [0, 1], got %r" % (ddim_eta,))
-    return {} if diffusion_sampler == "p" else {"sampler": diffusion_sampler, "eta": eta}
+    if diffusion_sampler == "p":
+        return {}
+    if diffusion_sampler == "ddim":
+        return {"sampler": "ddim", "eta": eta}
+    return {"sampler": diffusion_sampler}
 
 
 _CLASSIFIERS = {}
@@ -523,8 +528,9 @@ class TextToSpeech:
         `typical_sampling` / `typical_mass` are the reference's generate kwargs of the same names (api.py:361-364): the
         sampler keeps only the typical set of mass `typical_mass` (in (0, 1]) of the penalised scores.
         `diffusion_sampler` picks the diffusion decoder's sampler on the same respaced schedule: "p" (the reference's
-        p_sample_loop, the default) or "ddim" (its ddim_sample_loop, utils/diffusion.py:711-793) with `ddim_eta` in [0, 1]
-        (0: deterministic given x_T). Both draw the same noises from the same seed, so they start from the same x_T."""
+        p_sample_loop, the default), "ddim" (its ddim_sample_loop, utils/diffusion.py:711-793) with `ddim_eta` in [0, 1]
+        (0: deterministic given x_T) or "dpm++2m" (DPM-Solver++(2M), Lu et al. 2022; deterministic given x_T, `ddim_eta`
+        is checked and ignored). Every sampler draws the same noises from the same seed, so they start from the same x_T."""
         if hf_generate_kwargs:
             raise TypeError(f"unsupported generate kwargs: {sorted(hf_generate_kwargs)}")
         typical = _typical_mass(typical_sampling, typical_mass)

@@ -212,6 +212,39 @@ ddim_step_kernel(TtbDiffStepArgs a) {
   }
 }
 
+// DPM-Solver++(2M) step epilogue (Lu et al. 2022, Algorithm 2). One thread per (s, c). The learned-variance half of
+// model_out is not read. x0_prev [S, C] carries the clamped x0 of the previous call.
+__global__ void __launch_bounds__(256)
+dpmpp2m_step_kernel(TtbDiffStepArgs a, float* __restrict__ x0_prev) {
+  const long long idx = (long long)blockIdx.x * 256 + threadIdx.x;
+  if (idx >= (long long)a.S * a.C) return;
+  const int s = (int)(idx / a.C), c = (int)(idx - (long long)s * a.C);
+  const int call = *a.step;
+  const int i = a.iters - 1 - call;
+  const float* tb = a.tables;
+  const float sra = tb[0 * a.iters + i], srm1 = tb[1 * a.iters + i], ca = tb[2 * a.iters + i], cb = tb[3 * a.iters + i],
+              w = tb[4 * a.iters + i], wp = tb[5 * a.iters + i];
+  const float* mob = a.model_out + (long long)(call & 1) * a.parity_stride;
+  float eps = mob[(long long)s * a.ld_out + c];
+  if (a.cond_free) {
+    const float eps_u = mob[a.out_bstride + (long long)s * a.ld_out + c];
+    const double cfkd = (double)a.cond_free_k * (1.0 - (double)i / (double)a.iters);
+    eps = (float)(1.0 + cfkd) * eps - (float)cfkd * eps_u;
+  }
+  const float xt = a.x[idx];
+  const float d = fminf(fmaxf(sra * xt - srm1 * eps, -1.0f), 1.0f);
+  // a first-order step (wp == 0: first and last call) does not read x0_prev, which holds nothing of this chain yet
+  const float dm = (wp != 0.f) ? w * d + wp * x0_prev[idx] : w * d;
+  const float xn = ca * xt + cb * dm;
+  x0_prev[idx] = d;
+  a.x[idx] = xn;
+  if (a.x_bf16) reinterpret_cast<__nv_bfloat16*>(a.x_bf16)[(long long)s * a.ld_xb + c] = __float2bfloat16(xn);
+  if (a.mel_out && i == 0) {
+    const float MX = 2.3143386840820312f, MN = -11.512925148010254f;
+    a.mel_out[(long long)c * a.S + s] = ((xn + 1.0f) / 2.0f) * (MX - MN) + MN;
+  }
+}
+
 __global__ void counter_add_kernel(int* c, int d) { *c += d; }
 
 // ------------------------------------------------------------------ CFG pair: exchange of the two denoiser branches
@@ -331,6 +364,13 @@ extern "C" int ttb_ddim_step(const TtbDiffStepArgs* args, void* stream) {
   const long long n = (long long)args->S * args->C;
   ddim_step_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ST>>>(*args);
   TTB_CHECK_LAUNCH("ddim_step_kernel");
+  return 0;
+}
+extern "C" int ttb_dpmpp2m_step(const TtbDiffStepArgs* args, float* x0_prev, void* stream) {
+  if (!x0_prev) { set_error("ttb_dpmpp2m_step: x0_prev is required"); return -1; }
+  const long long n = (long long)args->S * args->C;
+  dpmpp2m_step_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ST>>>(*args, x0_prev);
+  TTB_CHECK_LAUNCH("dpmpp2m_step_kernel");
   return 0;
 }
 extern "C" int ttb_pair_exchange(const float* src, float* local_area, float* peer_area, long long n, long long parity_stride,

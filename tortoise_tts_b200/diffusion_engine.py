@@ -1,9 +1,9 @@
 """DiffusionTts denoiser + SpacedDiffusion sampling loop on the sm_90a kernels (hot loop 2, SURVEY §8 rows a9-a12).
 
 Mirrors `do_spectrogram_diffusion` (tortoise/api.py:117-130): `timestep_independent` once, then `iters` steps of
-p_sample (or ddim_sample with `sample(sampler="ddim")`) with the conditional and unconditional forward batched as B=2
-(the reference runs them sequentially, utils/diffusion.py:340-342), scheduler tables resident on the device and the
-whole step captured in one CUDA graph.
+p_sample (or ddim_sample with `sample(sampler="ddim")`, or DPM-Solver++(2M) with `sample(sampler="dpm++2m")`) with
+the conditional and unconditional forward batched as B=2 (the reference runs them sequentially,
+utils/diffusion.py:340-342), scheduler tables resident on the device and the whole step captured in one CUDA graph.
 Activations are token-major [B, S, C]; convolutions are wgmma GEMMs (k=3 as three shifted TMA loads).
 """
 import math
@@ -82,6 +82,32 @@ def make_ddim_schedule(iters, eta, trained_steps=4000):
     sigma = eta * np.sqrt((1.0 - ac_prev) / (1.0 - ac)) * np.sqrt(1.0 - ac / ac_prev)
     tables = np.stack([np.sqrt(1.0 / ac), np.sqrt(1.0 / ac - 1), np.sqrt(ac_prev),
                        np.sqrt(np.maximum(0.0, 1.0 - ac_prev - sigma ** 2)), sigma]).astype(np.float32)
+    return tmap, tables
+
+
+def make_dpmpp2m_schedule(iters, trained_steps=4000):
+    """The tables of the DPM-Solver++(2M) epilogue (Lu et al. 2022, arXiv:2211.01095, Algorithm 2) on the schedule of
+    make_schedule, built in float64 and rounded to fp32 once. Returns (timestep_map int64 [n], tables float32 [6, n]):
+    sqrt_recip_ac, sqrt_recipm1_ac, a, b, w, w_p. With alpha = sqrt(ac), sigma = sqrt(1 - ac),
+    lambda = log(alpha) - log(sigma) and spaced index i stepping to i - 1 (index -1 has ac = 1, lambda = +inf):
+    h_i = lambda_{i-1} - lambda_i, a = sigma_{i-1} / sigma_i, b = -alpha_{i-1} expm1(-h_i), r = h_{i+1} / h_i,
+    w = 1 + 1 / (2r), w_p = -1 / (2r). The first call (i = n - 1) is first order (w = 1, w_p = 0); the last (i = 0)
+    returns x' = D (a = 0, b = 1, w = 1, w_p = 0)."""
+    tmap, betas = _respace(iters, trained_steps)
+    ac = np.cumprod(1.0 - betas, axis=0)
+    ac_prev = np.append(1.0, ac[:-1])
+    n = len(tmap)
+    lam = 0.5 * (np.log(ac) - np.log(1.0 - ac))
+    h = np.full(n, np.inf)
+    h[1:] = lam[:-1] - lam[1:]
+    a, b = np.zeros(n), np.ones(n)
+    a[1:] = np.sqrt((1.0 - ac_prev[1:]) / (1.0 - ac[1:]))
+    b[1:] = -np.sqrt(ac_prev[1:]) * np.expm1(-h[1:])
+    w, w_p = np.ones(n), np.zeros(n)
+    r = h[2:] / h[1:-1]                     # indices 1 .. n-2: the calls between the first and the last
+    w[1:-1] = 1.0 + 0.5 / r
+    w_p[1:-1] = -0.5 / r
+    tables = np.stack([np.sqrt(1.0 / ac), np.sqrt(1.0 / ac - 1), a, b, w, w_p]).astype(np.float32)
     return tmap, tables
 
 
@@ -290,8 +316,18 @@ class DiffusionEngine:
         self._forward(st)
         self._epilogue(st)
 
-    def _epilogue(self, st):
+    def _scheduler_step(self, st, model_out, out_bstride, parity_stride=0):
+        """The sampler's scheduler epilogue on the model outputs of this call (both CFG branches)."""
+        if st["sampler"] == "dpm++2m":
+            lib.dpmpp2m_step(model_out, out_bstride, self.cout, st["x"], st["x_bf"], self.cin_pad, st["tables"],
+                             st["counter"], st["S"], self.cin, st["iters"], st["cond_free"], st["cond_free_k"],
+                             st["x0_prev"], st["mel"], parity_stride=parity_stride)
+            return
         step = lib.ddim_step if st["sampler"] == "ddim" else lib.diffusion_step
+        step(model_out, out_bstride, self.cout, st["x"], st["x_bf"], self.cin_pad, st["noise"], st["tables"], st["counter"],
+             st["S"], self.cin, st["iters"], st["cond_free"], st["cond_free_k"], st["mel"], parity_stride=parity_stride)
+
+    def _epilogue(self, st):
         xch = st.get("xch")
         if xch is not None:
             # CFG pair over peer memory: one captured launch puts my branch into both exchange areas and waits for the
@@ -299,8 +335,7 @@ class DiffusionEngine:
             n = st["S"] * self.cout
             lib.pair_exchange(st["mo_local"], xch.area, xch.peer_area, n, 2 * n, xch.my_idx * n, xch.peer_flags, xch.flags,
                               st["counter"], xch.epoch, xch.done, xch.err)
-            step(xch.area, n, self.cout, st["x"], st["x_bf"], self.cin_pad, st["noise"], st["tables"], st["counter"],
-                 st["S"], self.cin, st["iters"], st["cond_free"], st["cond_free_k"], st["mel"], parity_stride=2 * n)
+            self._scheduler_step(st, xch.area, n, parity_stride=2 * n)
             lib.counter_add(st["counter"], 1)
             return
         if st.get("pair") is not None:
@@ -312,14 +347,13 @@ class DiffusionEngine:
                 dist.all_gather_into_tensor(st["model_out"].view(-1), st["mo_local"].view(-1), group=st["pair"][0])
             else:   # gloo (CPU tests of the host logic)
                 dist.all_gather([st["model_out"][0], st["model_out"][1]], st["mo_local"][0], group=st["pair"][0])
-        step(st["model_out"], st["S"] * self.cout, self.cout, st["x"], st["x_bf"], self.cin_pad, st["noise"], st["tables"],
-             st["counter"], st["S"], self.cin, st["iters"], st["cond_free"], st["cond_free_k"], st["mel"])
+        self._scheduler_step(st, st["model_out"], st["S"] * self.cout)
         lib.counter_add(st["counter"], 1)
 
     def _state(self, S, B, iters, cfk=0.0, pair=None, sampler="p"):
         """B = number of CFG branches evaluated ON THIS RANK (2, or 1 when the pair is split over two GPUs / no CFG).
         The captured graph holds the sampler's epilogue, so the sampler is part of the key; DDIM's eta lives only in
-        st['tables']."""
+        st['tables']. DPM-Solver++(2M) keeps the previous call's clamped x0 in st['x0_prev'] (per rank)."""
         key = (S, B, iters, cfk, None if pair is None else pair[1], sampler)
         if self._ws is not None and self._ws["key"] == key:
             self._ws["pair"] = pair
@@ -339,6 +373,7 @@ class DiffusionEngine:
         st["tables"] = torch.empty(6, iters, dtype=torch.float32, device=dev)
         st["counter"] = torch.zeros(1, dtype=torch.int32, device=dev)
         st["mel"] = torch.empty(self.cin, S, dtype=torch.float32, device=dev)
+        st["x0_prev"] = torch.empty(S, self.cin, dtype=torch.float32, device=dev) if sampler == "dpm++2m" else None
         # per-ResBlock [scale | shift] rows for every step, in CALL order; the GroupNorm kernel indexes the row of the
         # current call with the device-side counter, so one captured graph serves every step
         st["ss_all"] = torch.empty(len(self.res_all), iters, 2 * C, dtype=torch.float32, device=dev)
@@ -388,6 +423,8 @@ class DiffusionEngine:
         noise0 [100, S] (already scaled by the temperature), step_noise [iters, 100, S] in call order.
         `sampler`: "p" runs p_sample_loop, "ddim" runs ddim_sample_loop with `eta` in [0, 1] (utils/diffusion.py:711-793)
         on the same respaced schedule and model call; DDIM reads step_noise[c] at call c too, scaled by sigma.
+        "dpm++2m" runs DPM-Solver++(2M) (make_dpmpp2m_schedule) on the same schedule; it reads no step noise and
+        ignores `eta`.
         Returns the denormalised mel fp32 [100, S] (channel-major, as the reference returns it)."""
         C, dev = self.C, self.dev
         N = latents.shape[0]
@@ -402,8 +439,10 @@ class DiffusionEngine:
             if not 0.0 <= eta <= 1.0:
                 raise ValueError("ddim eta must lie in [0, 1], got %r" % (eta,))
             tmap, tables = make_ddim_schedule(iters, float(eta))
+        elif sampler == "dpm++2m":
+            tmap, tables = make_dpmpp2m_schedule(iters)
         else:
-            raise ValueError("unknown diffusion sampler %r (expected 'p' or 'ddim')" % (sampler,))
+            raise ValueError("unknown diffusion sampler %r (expected 'p', 'ddim' or 'dpm++2m')" % (sampler,))
         n = len(tmap)
         st = self._state(S, B, n, float(cond_free_k), pair, sampler)
         st["cond_free"], st["cond_free_k"] = bool(cond_free), float(cond_free_k)

@@ -76,8 +76,8 @@ SYMBOLS = [
     "ttb_last_error", "ttb_version", "ttb_device_ok", "ttb_gemm", "ttb_layernorm", "ttb_rmsnorm", "ttb_groupnorm", "ttb_groupnorm_apply", "ttb_act_split_cast", "ttb_interp_linear",
     "ttb_residual_layernorm", "ttb_attention", "ttb_ar_embed_step", "ttb_ar_decode_attention", "ttb_ar_store_prefix", "ttb_ar_sample",
     "ttb_ar_fix_codes", "ttb_embed", "ttb_clvp_rotary", "ttb_clvp_pool", "ttb_clvp_project",
-    "ttb_timestep_embedding", "ttb_linear_small", "ttb_interp_nearest", "ttb_diffusion_step", "ttb_ddim_step", "ttb_counter_add",
-    "ttb_transpose_f32", "ttb_cast_pad_bf16", "ttb_broadcast_rows", "ttb_voc_conv1d", "ttb_voc_convt",
+    "ttb_timestep_embedding", "ttb_linear_small", "ttb_interp_nearest", "ttb_diffusion_step", "ttb_ddim_step", "ttb_dpmpp2m_step",
+    "ttb_counter_add", "ttb_transpose_f32", "ttb_cast_pad_bf16", "ttb_broadcast_rows", "ttb_voc_conv1d", "ttb_voc_convt",
     "ttb_voc_lvc_gate", "ttb_voc_to_tokens_bf16", "ttb_debug_gemm_trace",
     "ttb_ar_step_workspace", "ttb_ar_step_setup", "ttb_ar_decode_step", "ttb_ar_step_store_prefix",
     "ttb_audio_resample", "ttb_audio_stft_mel", "ttb_mean_rows", "ttb_equal_linear",
@@ -496,6 +496,20 @@ def ddim_step(model_out, out_bstride, ld_out, x, x_bf16, ld_xb, noise, tables, s
     a.S, a.C, a.iters, a.cond_free, a.cond_free_k = S, Cc, iters, 1 if cond_free else 0, cond_free_k
     a.mel_out = _p(_f32(mel_out)).value or 0
     _chk(load().ttb_ddim_step(C.byref(a), _stream()), "ttb_ddim_step")
+
+
+def dpmpp2m_step(model_out, out_bstride, ld_out, x, x_bf16, ld_xb, tables, step, S, Cc, iters, cond_free, cond_free_k,
+                 x0_prev, mel_out=None, parity_stride=0):
+    """The DPM-Solver++(2M) epilogue (include/ttb.h ttb_dpmpp2m_step): arguments as diffusion_step without `noise`,
+    `tables` from make_dpmpp2m_schedule, `x0_prev` fp32 [S, Cc] carries the clamped x0 from one call to the next."""
+    a = DiffStepArgs()
+    a.parity_stride = parity_stride
+    a.model_out, a.out_bstride, a.ld_out = _f32(model_out).data_ptr(), out_bstride, ld_out
+    a.x, a.x_bf16, a.ld_xb = _f32(x).data_ptr(), _p(_bf(x_bf16)).value or 0, ld_xb
+    a.noise, a.tables, a.step = 0, _f32(tables).data_ptr(), step.data_ptr()
+    a.S, a.C, a.iters, a.cond_free, a.cond_free_k = S, Cc, iters, 1 if cond_free else 0, cond_free_k
+    a.mel_out = _p(_f32(mel_out)).value or 0
+    _chk(load().ttb_dpmpp2m_step(C.byref(a), _p(_f32(x0_prev)), _stream()), "ttb_dpmpp2m_step")
 
 
 def counter_add(counter, delta):
